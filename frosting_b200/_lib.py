@@ -16,7 +16,7 @@ TILE = 16
 # every symbol include/frosting_b200.h declares
 EXPORTED = [
     "fb200_abi_version", "fb200_abi_struct_sizes", "fb200_last_error", "fb200_geom_bytes", "fb200_image_bytes",
-    "fb200_binning_bytes", "fb200_rec_stream_bytes", "fb200_forward", "fb200_forward_geometry", "fb200_forward_raster", "fb200_backward", "fb200_mark_visible",
+    "fb200_binning_bytes", "fb200_forward", "fb200_forward_geometry", "fb200_forward_raster", "fb200_backward", "fb200_mark_visible",
     "fb200_mesh_visibility", "fb200_gaussian_mask_from_faces", "fb200_get_layout",
     "fb200_profile_enable", "fb200_profile_read", "fb200_kernel_launches",
     "fb200_frosting_attributes", "fb200_frosting_attributes_backward",
@@ -24,7 +24,7 @@ EXPORTED = [
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
 NUM_STAGES = 5
-ABI_VERSION = 4
+ABI_VERSION = 5
 STAGES = ("preprocess", "binning", "render_fwd", "render_bwd", "geom_bwd")
 
 
@@ -60,7 +60,6 @@ class Workspace(C.Structure):
         ("d_status", C.c_void_p),
         ("acc_zeroed_by_forward", C.c_int32),
         ("h_status", C.c_void_p),
-        ("d_rec_stream", C.c_void_p), ("rec_stream_bytes", C.c_size_t),
     ]
 
 
@@ -130,12 +129,11 @@ def lib():
     L = C.CDLL(LIB_PATH)
     L.fb200_abi_version.restype = C.c_int
     L.fb200_last_error.restype = C.c_char_p
-    for n in ("fb200_geom_bytes", "fb200_image_bytes", "fb200_binning_bytes", "fb200_rec_stream_bytes"):
+    for n in ("fb200_geom_bytes", "fb200_image_bytes", "fb200_binning_bytes"):
         getattr(L, n).restype = C.c_size_t
     L.fb200_geom_bytes.argtypes = [C.c_int32]
     L.fb200_image_bytes.argtypes = [C.c_int32, C.c_int32]
     L.fb200_binning_bytes.argtypes = [C.c_int64]
-    L.fb200_rec_stream_bytes.argtypes = [C.c_int64]
     L.fb200_forward.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace),
                                 C.c_void_p, C.c_void_p, C.c_void_p]
     L.fb200_forward_geometry.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace),

@@ -83,6 +83,8 @@ int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_worksp
         return fail(FB200_EINVAL, "bad extents (P >= 0, image dims > 0 required)%s");
     if (prm->image_width > 65535 * FB200_TILE || prm->image_height > 65535 * FB200_TILE)
         return fail(FB200_EINVAL, "image too large for 16-bit tile coordinates%s");
+    if (prm->debug & ~3)
+        return fail(FB200_EINVAL, "debug: only bits 0 (synchronise) and 1 (no sub-tile culling) are defined%s");
     if (in->frosting) {
         int rc = validate_frosting(prm, in);
         if (rc != FB200_OK) return rc;
@@ -231,7 +233,6 @@ const char* fb200_last_error(void) { return g_err; }
 size_t fb200_geom_bytes(int32_t P) { return GeomLayout((size_t)(P < 0 ? 0 : P)).total; }
 size_t fb200_image_bytes(int32_t W, int32_t H) { return ImageLayout(W < 1 ? 1 : W, H < 1 ? 1 : H).total; }
 size_t fb200_binning_bytes(int64_t capacity) { return BinLayout((size_t)(capacity < 0 ? 0 : capacity)).total; }
-size_t fb200_rec_stream_bytes(int64_t capacity) { return (size_t)(capacity < 0 ? 0 : capacity) * sizeof(SplatRec) + 256; }
 
 int fb200_get_layout(int32_t P, int32_t W, int32_t H, int64_t capacity, fb200_layout* out) {
     if (!out || P < 0 || W <= 0 || H <= 0 || capacity < 0) return fail(FB200_EINVAL, "bad layout query%s");
@@ -287,12 +288,6 @@ static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb20
     a.keys_scratch = bn ? reinterpret_cast<unsigned long long*>(bn + bl.keys_scratch) : nullptr;
     a.sub_hits = bn ? reinterpret_cast<uint32_t*>(bn + bl.sub_hits) : nullptr;
     a.capacity = ws->binning_capacity;
-    a.rec_stream = nullptr;
-    if ((prm->debug & 8) && ws->d_rec_stream) {
-        if (ws->rec_stream_bytes < fb200_rec_stream_bytes(ws->binning_capacity))
-            return fail(FB200_ENOSPC, "record stream workspace too small%s");
-        a.rec_stream = reinterpret_cast<SplatRec*>(align128(ws->d_rec_stream));
-    }
     a.status = ws->d_status;
     a.out_color = d_out_color;
     a.radii = d_radii;
@@ -408,22 +403,8 @@ int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_
 
     if (!ws->acc_zeroed_by_forward &&
         (rc = stage(launch_render_bwd_clear(a, s), "render backward (clear)", debug, s)) != FB200_OK) return rc;
-    // the zero rows of the dense-gradient contract are written on a side stream while the blend backward runs
-    // (opt-in, debug bit 5: measured slower on C3 / C5 -- the fill kernel's CTAs take
-    // issue slots from the blend backward, which is issue-bound; kept for frames whose blend backward is short)
-    SideStream* side = (!grads->sparse_rows && !in->frosting && !debug && (prm->debug & 32) && prm->P >= 4096) ? side_stream() : nullptr;
-    std::unique_lock<std::mutex> side_use;
-    if (side) {
-        side_use = std::unique_lock<std::mutex>(side->use);
-        if ((rc = check(cudaEventRecord(side->fork, s), "fork")) != FB200_OK) return rc;
-        if ((rc = check(cudaStreamWaitEvent(side->stream, side->fork, 0), "fork")) != FB200_OK) return rc;
-        if ((rc = check(launch_zero_rows(a, side->stream), "zero rows")) != FB200_OK) return rc;
-        if ((rc = check(cudaEventRecord(side->join, side->stream), "join")) != FB200_OK) return rc;
-        a.zeroed_elsewhere = 1;
-    }
     { StageTimer t(FB200_STAGE_RENDER_BWD, s);
       if ((rc = stage(launch_render_bwd(a, s), "render backward", debug, s)) != FB200_OK) return rc; }
-    if (side && (rc = check(cudaStreamWaitEvent(s, side->join, 0), "join")) != FB200_OK) return rc;
     { StageTimer t(FB200_STAGE_GEOM_BWD, s);
       if ((rc = stage(launch_geom_bwd(a, s), "geometry backward", debug, s)) != FB200_OK) return rc; }
     if ((rc = stage(launch_extra_grad(a, s), "extra feature gradients", debug, s)) != FB200_OK) return rc;

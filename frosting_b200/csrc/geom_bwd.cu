@@ -84,20 +84,6 @@ __device__ __forceinline__ void zero_row(const BwdArgs& a, size_t i, int M) {
     }
 }
 
-// Opt-in (debug bit 5): the runs of 32 rows nobody rendered -- the bulk of the dense contract's zero rows under occlusion
-// culling -- zero-filled on a side stream while the blend backward runs; geom_bwd_kernel then skips them.
-__global__ void __launch_bounds__(256)
-zero_rows_kernel(BwdArgs a) {
-    const int lane = threadIdx.x & 31;
-    const long long warp_id = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
-    const int P = a.prm.P, M = a.prm.sh_coeffs;
-    for (long long g0 = warp_id * 32; g0 + 31 < P; g0 += n_warps * 32) {
-        const bool visible = a.radii[g0 + lane] > 0;
-        if (!__any_sync(0xffffffffu, visible)) zero_warp_rows(a, (size_t)g0, M, lane);
-    }
-}
-
 // ---- one row per lane <-> shared staging block, moved by the whole warp ----
 // A lane reading ITS row straight from global memory (12 x 128-bit at a 192-byte stride, or 45 scalars at 180 bytes
 // for Frosting's `rest` rows) costs 32 LSU wavefronts per instruction -- two to seven times the sectors the rows
@@ -240,10 +226,8 @@ geom_bwd_kernel(BwdArgs a) {
             active = in_rows && a.radii[idx] > 0;
             if (!__any_sync(full, active)) {
                 // nothing rendered in this run (the common case under occlusion culling): zeros, coalesced
-                if (!a.zeroed_elsewhere || rows < 32) {
-                    if (rows == 32) zero_warp_rows(a, (size_t)jb, M, lane);
-                    else if (in_rows) zero_row(a, (size_t)idx, M);
-                }
+                if (rows == 32) zero_warp_rows(a, (size_t)jb, M, lane);
+                else if (in_rows) zero_row(a, (size_t)idx, M);
                 continue;
             }
         }
@@ -576,15 +560,6 @@ geom_bwd_kernel(BwdArgs a) {
 }
 
 }  // namespace
-
-cudaError_t launch_zero_rows(const BwdArgs& a, cudaStream_t s) {
-    if (a.prm.P >= 32) {
-        // HBM-bound stores beside the blend backward: one CTA per SM keeps HBM busy without taking that kernel's warp slots
-        zero_rows_kernel<<<sm_count(), 256, 0, s>>>(a);
-        count_launch();
-    }
-    return cudaGetLastError();
-}
 
 cudaError_t launch_geom_bwd(const BwdArgs& a, cudaStream_t s) {
     if (a.prm.P > 0) {

@@ -1,17 +1,18 @@
-// render_bwd.cu -- backward of the alpha compositing, warp-autonomous, two Gaussians per lane-iteration.
+// render_bwd.cu -- backward of the alpha compositing, warp-autonomous: one warp per 8x4-pixel sub-tile, no CTA barrier
+// (staging 256-instance batches cooperatively was dominated by barrier stalls).
 //
 // Replaces renderCUDA<3> backward (DGR/cuda_rasterizer/backward.cu:399-557): back-to-front traversal from each
 // pixel's last contributor, T recovered by division, gradients w.r.t. the per-Gaussian 2D mean, conic, opacity and
-// colour.  Same formulas; structure:
-//   * the reference issues 9 global float atomics per contributing PIXEL-Gaussian pair (its dominant cost).  Here a
-//     warp (8x4 pixels) sums its 32 lanes' contributions with a transposing butterfly and issues ONE red.global.add
-//     instruction per PAIR of Gaussians (18 active lanes, addresses inside two 48-byte accumulator records);
-//   * every warp walks the list on its own, 32 instances per step, starting at ITS deepest last contributor; no CTA
-//     barrier (staging 256-instance batches cooperatively was dominated by barrier stalls).  Records re-read by the
-//     warps of a tile are L1/L2 hits;
-//   * the same conservative alpha>=1/255 extents as the forward kernel let a warp skip instances that cannot touch
-//     its sub-tile;
-//   * instruction-issue bound, hence pairs of hits sharing the per-pixel operands (kernel comment below).
+// colour.  Same formulas.  The reference issues 9 global float atomics per contributing PIXEL-Gaussian pair (its
+// dominant cost); here a warp sums its 32 pixels' contributions before it touches the accumulators.  Two kernels,
+// both instruction-issue bound, chosen by launch_render_bwd:
+//   * render_bwd_t16_kernel serves every frame without extra channels.  It walks the sub-tile hit list the forward
+//     blend wrote, in blocks of 16 Gaussians: lane = Gaussian for the per-pair math, lane = pixel for the
+//     recurrences (kernel comment below);
+//   * render_bwd_pair_kernel serves extra feature channels (fb200_extra).  It walks the tile's instance list, 32
+//     instances per step from the warp's deepest last contributor, skips instances whose conservative alpha>=1/255
+//     extents miss the sub-tile, and evaluates two Gaussians per lane-iteration, lane = pixel throughout (kernel
+//     comment below).  Records re-read by the warps of a tile are L1/L2 hits.
 #include "common.cuh"
 
 namespace fb200 {
@@ -22,14 +23,14 @@ __device__ __forceinline__ bool overlaps(float lo, float hi, float c, float ext)
     return !(c + ext < lo) && !(c - ext > hi);
 }
 
-// ---- two Gaussians per lane-iteration --------------------------------------------------------------------------------
+// ---- extra channels: two Gaussians per lane-iteration ----------------------------------------------------------------
 // The per-warp hit records of a step are COMPACTED into a structure-of-arrays slab (slot = rank of the lane among the
 // hits), so hits 2k and 2k+1 sit in adjacent words and one 64-bit shared load yields an aligned register pair; the
 // alpha evaluation (libdevice-exact exp included) and the gradient algebra then run as pair operations (common.cuh P2)
 // on (Gaussian 2k, Gaussian 2k+1).  Only the transmittance / accum_rec recurrences, which chain through the two
-// Gaussians at a pixel, stay scalar.  The 18 partial gradients (2 x 9) of the pair are summed over the warp by ONE
-// transposing butterfly -- 16 values fold 16->8->4->2->1 over lane bits 4..1, the two blue-channel values ride along --
-// in 20 shuffles, and ONE red.global.add instruction (18 lanes) retires both Gaussians.
+// Gaussians at a pixel, stay scalar.  The 24 partial gradients (2 x 12) of the pair are summed over the warp by ONE
+// transposing butterfly -- 16 values fold 16->8->4->2->1 over lane bits 4..1, the blue-channel and extra-channel values
+// ride along -- in 24 shuffles, and ONE red.global.add instruction (24 lanes) retires both Gaussians.
 struct __align__(16) PairSlab {
     float x[34], y[34], A[34], B[34], C[34], op[34], r[34], g[34], b[34];
     uint32_t id[34], pos[34];
@@ -40,10 +41,8 @@ struct __align__(16) PairSlabX {
 
 __device__ __forceinline__ P2 ldp(const float* a, int k) { return *reinterpret_cast<const float2*>(a + k); }
 
-// 80 registers / 24 resident warps per SM (72 / 28 and 64 / 32 cost more instructions; the kernel is issue-bound, not
-// latency-bound)
-template <bool kExtra, int kWarps>
-__global__ void __launch_bounds__(32 * kWarps, (kExtra ? 16 : 24) / kWarps)
+template <int kWarps>
+__global__ void __launch_bounds__(32 * kWarps, 16 / kWarps)
 render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                        const SplatRec* __restrict__ rec, int W, int H, int tiles_x,
                        const float* __restrict__ bg, const float* __restrict__ final_T,
@@ -51,7 +50,7 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
                        float* __restrict__ acc, const int32_t* __restrict__ status, const ExtraArgs ex,
                        const uint32_t* __restrict__ tile_order) {
     __shared__ PairSlab slabs[kWarps];
-    __shared__ PairSlabX slabs_x[kExtra ? kWarps : 1];
+    __shared__ PairSlabX slabs_x[kWarps];
     if (status[FB200_ST_OVERFLOW]) return;
 
     const unsigned full = 0xffffffffu;
@@ -66,11 +65,11 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
     asm volatile("mov.u32 %0, %%lanemask_lt;" : "=r"(lt_mask));
     const bool lb4 = lane & 16, lb3 = lane & 8, lb2 = lane & 4, lb1 = lane & 2, lb0 = lane & 1;
     // after the butterfly: even lanes hold value (lane >> 1) & 7 of Gaussian (lane >> 4); odd lanes hold the ride-along
-    // values: slot 8 (kExtra: 8 + ((lane >> 2) & 3)) of Gaussian (lane >> 4)
-    const bool red_lane = !lb0 || (kExtra ? (lane & 3) == 1 : (lane & 15) == 1);
-    const int red_slot = lb0 ? (kExtra ? 8 + ((lane >> 2) & 3) : 8) : ((lane >> 1) & 7);
+    // values: slot 8 + ((lane >> 2) & 3) of Gaussian (lane >> 4)
+    const bool red_lane = !lb0 || (lane & 3) == 1;
+    const int red_slot = lb0 ? 8 + ((lane >> 2) & 3) : ((lane >> 1) & 7);
     PairSlab& slab = slabs[wslot];
-    PairSlabX& slabx = slabs_x[kExtra ? wslot : 0];
+    PairSlabX& slabx = slabs_x[wslot];
     const int sub_x0 = tile_x * kTile + (warp & 1) * kSubW;
     const int sub_y0 = tile_y * kTile + (warp >> 1) * kSubH;
     const int pix_x = sub_x0 + (lane & 7), pix_y = sub_y0 + (lane >> 3);
@@ -93,16 +92,14 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
     }
     float bg_dot_dpixel = bg[0] * dp0 + bg[1] * dp1 + bg[2] * dp2;
     float de0 = 0.f, de1 = 0.f, de2 = 0.f;
-    if (kExtra) {
-        if (inside) {
-            de0 = ex.dL_dout[pix_id];
-            if (ex.ch > 1) de1 = ex.dL_dout[HW + pix_id];
-            if (ex.ch > 2) de2 = ex.dL_dout[2 * HW + pix_id];
-        }
-        bg_dot_dpixel += ex.bg[0] * de0;
-        if (ex.ch > 1) bg_dot_dpixel += ex.bg[1] * de1;
-        if (ex.ch > 2) bg_dot_dpixel += ex.bg[2] * de2;
+    if (inside) {
+        de0 = ex.dL_dout[pix_id];
+        if (ex.ch > 1) de1 = ex.dL_dout[HW + pix_id];
+        if (ex.ch > 2) de2 = ex.dL_dout[2 * HW + pix_id];
     }
+    bg_dot_dpixel += ex.bg[0] * de0;
+    if (ex.ch > 1) bg_dot_dpixel += ex.bg[1] * de1;
+    if (ex.ch > 2) bg_dot_dpixel += ex.bg[2] * de2;
     const float ddelx_dx = 0.5f * W, ddely_dy = 0.5f * H;
 
     const int n = (int)__reduce_max_sync(full, last_contributor);
@@ -126,7 +123,7 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
         id_cur = point_list[range.x + (n - 1 - lane)];
         const float4* p = reinterpret_cast<const float4*>(rec + id_cur);
         r0 = __ldg(p); r1 = __ldg(p + 1); r2 = __ldg(p + 2);
-        if (kExtra) load_extra(id_cur);
+        load_extra(id_cur);
     }
     if (32 + lane < n) id_next = point_list[range.x + (n - 1 - 32 - lane)];
 
@@ -140,20 +137,20 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
             slab.C[slot] = r1.x; slab.op[slot] = r1.y; slab.r[slot] = r1.z; slab.g[slot] = r1.w; slab.b[slot] = r2.x;
             slab.id[slot] = id_cur;
             slab.pos[slot] = (uint32_t)(n - 1 - base - lane);
-            if (kExtra) { slabx.e0[slot] = x0; slabx.e1[slot] = x1; slabx.e2[slot] = x2; }
+            slabx.e0[slot] = x0; slabx.e1[slot] = x1; slabx.e2[slot] = x2;
         }
         if ((nhit & 1) && lane == 0) {
             // odd count: pad with a record that can never contribute (opacity 0, position beyond every pixel's last)
             slab.x[nhit] = 0.f; slab.y[nhit] = 0.f; slab.A[nhit] = 0.f; slab.B[nhit] = 0.f; slab.C[nhit] = 0.f;
             slab.op[nhit] = 0.f; slab.r[nhit] = 0.f; slab.g[nhit] = 0.f; slab.b[nhit] = 0.f;
             slab.id[nhit] = 0u; slab.pos[nhit] = 0xffffffffu;
-            if (kExtra) { slabx.e0[nhit] = 0.f; slabx.e1[nhit] = 0.f; slabx.e2[nhit] = 0.f; }
+            slabx.e0[nhit] = 0.f; slabx.e1[nhit] = 0.f; slabx.e2[nhit] = 0.f;
         }
         id_cur = id_next;
         if (base + 32 + lane < n) {
             const float4* p = reinterpret_cast<const float4*>(rec + id_cur);
             r0 = __ldg(p); r1 = __ldg(p + 1); r2 = __ldg(p + 2);
-            if (kExtra) load_extra(id_cur);
+            load_extra(id_cur);
         }
         if (base + 64 + lane < n) id_next = point_list[range.x + (n - 1 - base - 64 - lane)];
         __syncwarp();
@@ -192,31 +189,27 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
             // one right after use is the same arithmetic one step earlier and needs no last_alpha / last_color
             P2 AR0, AR1, AR2, TP, AE0, AE1, AE2;
             AR0.x = ar0; AR1.x = ar1; AR2.x = ar2;
-            if (kExtra) { AE0.x = ae0; AE1.x = ae1; AE2.x = ae2; }
+            AE0.x = ae0; AE1.x = ae1; AE2.x = ae2;
             if (act0) {
                 T = T * INV.x;
                 ar0 = al0 * Rc.x + om.x * ar0;
                 ar1 = al0 * Gc.x + om.x * ar1;
                 ar2 = al0 * Bc.x + om.x * ar2;
-                if (kExtra) {
-                    ae0 = al0 * slabx.e0[k] + om.x * ae0;
-                    ae1 = al0 * slabx.e1[k] + om.x * ae1;
-                    ae2 = al0 * slabx.e2[k] + om.x * ae2;
-                }
+                ae0 = al0 * slabx.e0[k] + om.x * ae0;
+                ae1 = al0 * slabx.e1[k] + om.x * ae1;
+                ae2 = al0 * slabx.e2[k] + om.x * ae2;
             }
             TP.x = T;
             AR0.y = ar0; AR1.y = ar1; AR2.y = ar2;
-            if (kExtra) { AE0.y = ae0; AE1.y = ae1; AE2.y = ae2; }
+            AE0.y = ae0; AE1.y = ae1; AE2.y = ae2;
             if (act1) {
                 T = T * INV.y;
                 ar0 = al1 * Rc.y + om.y * ar0;
                 ar1 = al1 * Gc.y + om.y * ar1;
                 ar2 = al1 * Bc.y + om.y * ar2;
-                if (kExtra) {
-                    ae0 = al1 * slabx.e0[k + 1] + om.y * ae0;
-                    ae1 = al1 * slabx.e1[k + 1] + om.y * ae1;
-                    ae2 = al1 * slabx.e2[k + 1] + om.y * ae2;
-                }
+                ae0 = al1 * slabx.e0[k + 1] + om.y * ae0;
+                ae1 = al1 * slabx.e1[k + 1] + om.y * ae1;
+                ae2 = al1 * slabx.e2[k + 1] + om.y * ae2;
             }
             TP.y = T;
 
@@ -226,14 +219,11 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
             const P2 dch = mul2(al, TP);                                       // d(channel)/d(colour)
             P2 dLa = fma2(add2(Rc, neg2(AR0)), bc(dp0),
                           fma2(add2(Gc, neg2(AR1)), bc(dp1), mul2(add2(Bc, neg2(AR2)), bc(dp2))));
-            P2 V9, V10, V11;
-            if (kExtra) {
-                const P2 F0 = ldp(slabx.e0, k), F1 = ldp(slabx.e1, k), F2 = ldp(slabx.e2, k);
-                dLa = fma2(add2(F0, neg2(AE0)), bc(de0), dLa);
-                dLa = fma2(add2(F1, neg2(AE1)), bc(de1), dLa);
-                dLa = fma2(add2(F2, neg2(AE2)), bc(de2), dLa);
-                V9 = mul2(dch, bc(de0)); V10 = mul2(dch, bc(de1)); V11 = mul2(dch, bc(de2));
-            }
+            const P2 F0 = ldp(slabx.e0, k), F1 = ldp(slabx.e1, k), F2 = ldp(slabx.e2, k);
+            dLa = fma2(add2(F0, neg2(AE0)), bc(de0), dLa);
+            dLa = fma2(add2(F1, neg2(AE1)), bc(de1), dLa);
+            dLa = fma2(add2(F2, neg2(AE2)), bc(de2), dLa);
+            const P2 V9 = mul2(dch, bc(de0)), V10 = mul2(dch, bc(de1)), V11 = mul2(dch, bc(de2));
             dLa = mul2(dLa, TP);
             dLa = fma2(mul2(bc(-T_final), INV), bc(bg_dot_dpixel), dLa);
             const P2 dL_dG = mul2(OP, dLa);
@@ -286,7 +276,7 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
             }
             // ride-along values
             float h;
-            if (kExtra) {
+            {
                 const P2 L[4] = {V8, V9, V10, V11};
                 float f[4];
 #pragma unroll
@@ -307,13 +297,6 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
                     const float keep = lb2 ? gq[1] : gq[0];
                     h = keep + __shfl_xor_sync(full, send, 4);   // ride-along 2*b3 + b2 of Gaussian b4
                 }
-                h += __shfl_xor_sync(full, h, 2);
-            } else {
-                const float send = lb4 ? V8.x : V8.y;
-                const float keep = lb4 ? V8.y : V8.x;
-                h = keep + __shfl_xor_sync(full, send, 16);
-                h += __shfl_xor_sync(full, h, 8);
-                h += __shfl_xor_sync(full, h, 4);
                 h += __shfl_xor_sync(full, h, 2);
             }
             float red;
@@ -366,8 +349,9 @@ struct __align__(16) BwdWarpSmem {
 // that passed the sub-tile test, in tile-list order, and per pixel the number of entries up to its last contributor.
 // The backward therefore touches no instance the forward did not blend into this sub-tile: no re-test, no walk over
 // the other 7/8 of the tile list, and the per-pixel "before my last contributor" test is a compare of entry numbers.
-template <int kWarps, int kResidentWarps>
-__global__ void __launch_bounds__(32 * kWarps, kResidentWarps / kWarps)
+// 20 resident warps per SM: 96 registers, no spills (24 warps at 80 registers measured slower)
+template <int kWarps>
+__global__ void __launch_bounds__(32 * kWarps, 20 / kWarps)
 render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ sub_hits,
                       const SplatRec* __restrict__ rec, int W, int H, int tiles_x,
                       const float* __restrict__ bg, const float* __restrict__ final_T,
@@ -624,19 +608,11 @@ cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s) {
     const int grid = T * (kWarpsPerTile / kWarps);
     count_launch();
     if (a.ex.ch > 0)
-        render_bwd_pair_kernel<true, kWarps><<<grid, 32 * kWarps, 0, s>>>(
+        render_bwd_pair_kernel<kWarps><<<grid, 32 * kWarps, 0, s>>>(
             a.ranges, a.point_list, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
             a.final_T, a.n_contrib, a.dL_dpix, a.acc, a.status, a.ex, a.tile_order);
-    else if (a.prm.debug & 4)       // A/B switch: the round-1 pair kernel (lane = pixel + butterfly)
-        render_bwd_pair_kernel<false, kWarps><<<grid, 32 * kWarps, 0, s>>>(
-            a.ranges, a.point_list, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
-            a.final_T, a.n_contrib, a.dL_dpix, a.acc, a.status, a.ex, a.tile_order);
-    else if (a.prm.debug & 16)      // A/B switch: 24 resident warps (80 registers) -- measured slower
-        render_bwd_t16_kernel<kWarps, 24><<<grid, 32 * kWarps, 0, s>>>(
-            a.ranges, a.sub_hits, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
-            a.final_T, a.last_entry, a.dL_dpix, a.acc, a.status, a.tile_order);
-    else                            // 20 resident warps per SM, 96 registers, no spills
-        render_bwd_t16_kernel<kWarps, 20><<<grid, 32 * kWarps, 0, s>>>(
+    else
+        render_bwd_t16_kernel<kWarps><<<grid, 32 * kWarps, 0, s>>>(
             a.ranges, a.sub_hits, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
             a.final_T, a.last_entry, a.dL_dpix, a.acc, a.status, a.tile_order);
     return cudaGetLastError();

@@ -44,12 +44,6 @@ NO_CULL = False   # test hook: disable sub-tile culling (debug bit 1) to prove i
 # FB200_EXACT_BINNING=1: always size the binning buffer from this frame's own instance count (two-phase forward with a
 # host wait, like the reference's blocking copy at rasterizer_impl.cu:280-281) instead of speculating from earlier frames
 EXACT_BINNING = os.environ.get("FB200_EXACT_BINNING", "0") == "1"
-# FB200_BWD_PAIR=1: A/B switch, blend backward through the round-1 pair kernel (debug bit 2)
-BWD_PAIR_KERNEL = os.environ.get("FB200_BWD_PAIR", "0") == "1"
-# FB200_FWD_TMA=1: A/B switch, forward blend staged by 1-D cp.async.bulk copies of a packed record stream (debug bit 3)
-FWD_TMA = os.environ.get("FB200_FWD_TMA", "0") == "1"
-ZERO_OVERLAP = os.environ.get("FB200_ZERO_OVERLAP", "0") == "1"   # A/B: dense zero rows on a side stream under the blend bwd (bit 5)
-BWD_OCC24 = os.environ.get("FB200_BWD_OCC24", "0") == "1"      # A/B: backward blend at 24 resident warps / SM (debug bit 4)
 # FB200_CHECK_BEFORE_BACKWARD=1: wait for a speculatively launched forward's status words before launching its backward
 # (an overflow is then raised from backward()).  Default: no wait -- the backward is enqueued behind the forward at once
 # (its kernels exit on the overflow word; the gradients of such a frame are zeros) and the overflow is raised by the next
@@ -263,7 +257,7 @@ def _prepare(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_p
     prm = Params(P=P, sh_degree=int(rs.sh_degree), sh_coeffs=int(M), image_width=W, image_height=H,
                  tanfovx=float(rs.tanfovx), tanfovy=float(rs.tanfovy),
                  scale_modifier=float(rs.scale_modifier), prefiltered=int(bool(rs.prefiltered)),
-                 debug=int(bool(rs.debug)) | (2 if NO_CULL else 0) | (4 if BWD_PAIR_KERNEL else 0) | (8 if FWD_TMA else 0) | (16 if BWD_OCC24 else 0) | (32 if ZERO_OVERLAP else 0), extra=None)
+                 debug=int(bool(rs.debug)) | (2 if NO_CULL else 0), extra=None)
     inp = Inputs(d_background=_ptr(bg), d_means3D=_ptr(means3D), d_shs=_ptr(sh),
                  d_colors_precomp=_ptr(colors_precomp), d_opacities=_ptr(opacities), d_scales=_ptr(scales),
                  d_rotations=_ptr(rotations), d_cov3D_precomp=_ptr(cov3Ds_precomp),
@@ -288,20 +282,10 @@ def _prepare_frosting(frosting, rs):
     prm = Params(P=P, sh_degree=int(rs.sh_degree), sh_coeffs=M, image_width=W, image_height=H,
                  tanfovx=float(rs.tanfovx), tanfovy=float(rs.tanfovy),
                  scale_modifier=float(rs.scale_modifier), prefiltered=int(bool(rs.prefiltered)),
-                 debug=int(bool(rs.debug)) | (2 if NO_CULL else 0) | (4 if BWD_PAIR_KERNEL else 0) | (16 if BWD_OCC24 else 0),
-                 extra=None)
+                 debug=int(bool(rs.debug)) | (2 if NO_CULL else 0), extra=None)
     inp = Inputs(d_background=_ptr(bg), d_viewmatrix=_ptr(view), d_projmatrix=_ptr(proj), d_campos=_ptr(campos),
                  n_cell_points=0, frosting=C.addressof(fp))
     return device, P, W, H, prm, inp, (fp, keep, bg, view, proj, campos), None, None
-
-
-def _attach_stream(L, ws, capacity, device):
-    """TMA A/B only: the packed record stream workspace (48 B per tile instance)."""
-    if not FWD_TMA:
-        return None
-    buf = torch.empty((L.fb200_rec_stream_bytes(capacity),), dtype=torch.uint8, device=device)
-    ws.d_rec_stream, ws.rec_stream_bytes = buf.data_ptr(), buf.numel()
-    return buf
 
 
 def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -366,7 +350,6 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
             if not geometry_only:
                 binning = torch.empty((L.fb200_binning_bytes(capacity),), dtype=torch.uint8, device=device)
                 ws.d_binning, ws.binning_bytes, ws.binning_capacity = binning.data_ptr(), binning.numel(), capacity
-                stream_buf = _attach_stream(L, ws, capacity, device)
                 ws.h_status = mailbox.data_ptr()     # the host HAS this frame's status words: empty sort classes are skipped
                 _lib.check(L.fb200_forward_raster(C.byref(prm), C.byref(inp), C.byref(ws),
                                                   C.c_void_p(out_color.data_ptr()), rptr, sptr))
@@ -377,7 +360,6 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
             capacity = hint
             binning = torch.empty((L.fb200_binning_bytes(capacity),), dtype=torch.uint8, device=device)
             ws.d_binning, ws.binning_bytes, ws.binning_capacity = binning.data_ptr(), binning.numel(), capacity
-            stream_buf = _attach_stream(L, ws, capacity, device)
             _lib.check(L.fb200_forward(C.byref(prm), C.byref(inp), C.byref(ws), C.c_void_p(out_color.data_ptr()),
                                        rptr, sptr))
             mailbox.copy_(status, non_blocking=True)

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define FB200_ABI_VERSION 4
+#define FB200_ABI_VERSION 5
 
 #define FB200_OK 0
 #define FB200_EINVAL (-1)   /* bad argument (shape / null pointer / unsupported channel count) */
@@ -72,7 +72,9 @@ typedef struct fb200_params {
     float tanfovy;
     float scale_modifier;
     int32_t prefiltered;     /* trap if a Gaussian is near-culled (auxiliary.h:156-160) */
-    int32_t debug;           /* synchronise + check after every stage */
+    int32_t debug;           /* bit 0: synchronise + check after every stage.  bit 1: disable sub-tile culling, every
+                                tile instance is evaluated in all 8 sub-tiles of its tile (slower; outputs identical).
+                                Any other bit set: FB200_EINVAL */
     const fb200_extra* extra; /* NULL: colour only (the reference's surface) */
 } fb200_params;
 
@@ -163,10 +165,6 @@ typedef struct fb200_workspace {
     const int32_t* h_status;               /* optional HOST copy of the status words written by fb200_forward_geometry,
                                               read by the caller after synchronising the stream; fb200_forward_raster
                                               then skips launches it can tell are empty.  NULL: launch for the worst case */
-    void* d_rec_stream; size_t rec_stream_bytes;  /* optional, fb200_rec_stream_bytes(binning_capacity): when given (and
-                                              prm->debug bit 3 is set) the forward blend runs the TMA-staged variant -- a
-                                              packed 48-byte record stream in sorted order, staged into shared memory
-                                              by 1-D cp.async.bulk copies (BASELINE north star; an A/B switch) */
 } fb200_workspace;
 
 /* d_status words written by fb200_forward (stream-ordered; copy back after the call). */
@@ -179,7 +177,6 @@ typedef struct fb200_workspace {
 size_t fb200_geom_bytes(int32_t P);
 size_t fb200_image_bytes(int32_t image_width, int32_t image_height);
 size_t fb200_binning_bytes(int64_t capacity);
-size_t fb200_rec_stream_bytes(int64_t capacity);
 
 /* Forward: preprocess + cull, per-tile bin/sort, front-to-back blend.
  *   d_out_color [3,H,W] f32, d_radii [P] i32 -- both fully written (no zero-fill needed).

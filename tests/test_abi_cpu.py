@@ -23,7 +23,7 @@ def test_every_declared_symbol_is_exported():
     for n in names:
         assert hasattr(L, n), f"{n} declared in the header but not exported"
     assert sorted(_lib.EXPORTED) == names, "frosting_b200/_lib.py:EXPORTED out of sync with the header"
-    assert L.fb200_abi_version() == _lib.ABI_VERSION == 4
+    assert L.fb200_abi_version() == _lib.ABI_VERSION == 5
 
 
 def test_workspace_size_queries_are_host_only_and_monotonic():
@@ -71,6 +71,11 @@ def test_argument_errors_are_reported_without_touching_cuda():
     assert rc == -1 and b"exactly one of either scale/rotation pair" in L.fb200_last_error()
     with pytest.raises(_lib.Fb200Error):
         _lib.check(rc)
+    # debug has two defined bits (sync, no sub-tile culling); any other bit is an error, not the default kernels
+    prm.debug = 8
+    rc = L.fb200_forward(C.byref(prm), C.byref(inp), C.byref(ws), None, None, None)
+    assert rc == -1 and b"debug" in L.fb200_last_error()
+    prm.debug = 0
     # frosting mode: the parameter block replaces the attribute pointers, it does not coexist with them
     d = dummy
     fp = _lib.FrostingParams(P=10, n_verts=4, n_faces=2, sh_rest=15, d_bary_logits=d, d_cells=d, d_faces=d, d_inner_verts=d,
