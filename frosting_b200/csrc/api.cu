@@ -389,11 +389,9 @@ int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_
     a.vis_list = reinterpret_cast<const uint32_t*>(g + gl.vis_list);
     a.acc = reinterpret_cast<float*>(g + gl.acc);
     a.final_T = reinterpret_cast<const float*>(im + il.final_T);
-    a.n_contrib = reinterpret_cast<const uint32_t*>(im + il.n_contrib);
     a.last_entry = reinterpret_cast<const uint32_t*>(im + il.last_entry);
     a.tile_order = reinterpret_cast<const uint32_t*>(im + il.tile_order);
     a.ranges = reinterpret_cast<const uint2*>(im + il.ranges);
-    a.point_list = bn ? reinterpret_cast<const uint32_t*>(bn + bl.point_list) : nullptr;
     a.sub_hits = bn ? reinterpret_cast<const uint32_t*>(bn + bl.sub_hits) : nullptr;
     a.status = ws->d_status;
     a.radii = d_radii;

@@ -4,321 +4,23 @@
 // Replaces renderCUDA<3> backward (DGR/cuda_rasterizer/backward.cu:399-557): back-to-front traversal from each
 // pixel's last contributor, T recovered by division, gradients w.r.t. the per-Gaussian 2D mean, conic, opacity and
 // colour.  Same formulas.  The reference issues 9 global float atomics per contributing PIXEL-Gaussian pair (its
-// dominant cost); here a warp sums its 32 pixels' contributions before it touches the accumulators.  Two kernels,
-// both instruction-issue bound, chosen by launch_render_bwd:
-//   * render_bwd_t16_kernel serves every frame without extra channels.  It walks the sub-tile hit list the forward
-//     blend wrote, in blocks of 16 Gaussians: lane = Gaussian for the per-pair math, lane = pixel for the
-//     recurrences (kernel comment below);
-//   * render_bwd_pair_kernel serves extra feature channels (fb200_extra).  It walks the tile's instance list, 32
-//     instances per step from the warp's deepest last contributor, skips instances whose conservative alpha>=1/255
-//     extents miss the sub-tile, and evaluates two Gaussians per lane-iteration, lane = pixel throughout (kernel
-//     comment below).  Records re-read by the warps of a tile are L1/L2 hits.
+// dominant cost); here a warp sums its 32 pixels' contributions before it touches the accumulators.  One kernel,
+// render_bwd_t16_kernel, instruction-issue bound: it walks the sub-tile hit list the forward blend wrote, in blocks of
+// 16 Gaussians, lane = Gaussian for the per-pair math, lane = pixel for the recurrences (kernel comment below).  Extra
+// feature channels (fb200_extra) are its kExtra instance: they widen the per-pair dot product with dL/dpixel by the
+// features' dot product with dL/dextra, and add one gradient sum per channel.
 #include "common.cuh"
 
 namespace fb200 {
 
 namespace {
 
-__device__ __forceinline__ bool overlaps(float lo, float hi, float c, float ext) {
-    return !(c + ext < lo) && !(c - ext > hi);
-}
-
-// ---- extra channels: two Gaussians per lane-iteration ----------------------------------------------------------------
-// The per-warp hit records of a step are COMPACTED into a structure-of-arrays slab (slot = rank of the lane among the
-// hits), so hits 2k and 2k+1 sit in adjacent words and one 64-bit shared load yields an aligned register pair; the
-// alpha evaluation (libdevice-exact exp included) and the gradient algebra then run as pair operations (common.cuh P2)
-// on (Gaussian 2k, Gaussian 2k+1).  Only the transmittance / accum_rec recurrences, which chain through the two
-// Gaussians at a pixel, stay scalar.  The 24 partial gradients (2 x 12) of the pair are summed over the warp by ONE
-// transposing butterfly -- 16 values fold 16->8->4->2->1 over lane bits 4..1, the blue-channel and extra-channel values
-// ride along -- in 24 shuffles, and ONE red.global.add instruction (24 lanes) retires both Gaussians.
-struct __align__(16) PairSlab {
-    float x[34], y[34], A[34], B[34], C[34], op[34], r[34], g[34], b[34];
-    uint32_t id[34], pos[34];
-};
-struct __align__(16) PairSlabX {
-    float e0[34], e1[34], e2[34];
-};
-
 __device__ __forceinline__ P2 ldp(const float* a, int k) { return *reinterpret_cast<const float2*>(a + k); }
 
-template <int kWarps>
-__global__ void __launch_bounds__(32 * kWarps, 16 / kWarps)
-render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
-                       const SplatRec* __restrict__ rec, int W, int H, int tiles_x,
-                       const float* __restrict__ bg, const float* __restrict__ final_T,
-                       const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dpix,
-                       float* __restrict__ acc, const int32_t* __restrict__ status, const ExtraArgs ex,
-                       const uint32_t* __restrict__ tile_order) {
-    __shared__ PairSlab slabs[kWarps];
-    __shared__ PairSlabX slabs_x[kWarps];
-    if (status[FB200_ST_OVERFLOW]) return;
-
-    const unsigned full = 0xffffffffu;
-    constexpr int kSplit = kWarpsPerTile / kWarps;
-    const int tile = (int)tile_order[blockIdx.x / kSplit];       // longest lists first (binning.cu)
-    const int tile_x = tile % tiles_x, tile_y = tile / tiles_x;
-    const int wslot = threadIdx.x >> 5;
-    const int warp = (blockIdx.x % kSplit) * kWarps + wslot;      // sub-tile index inside the tile
-    int lane;
-    unsigned lt_mask;
-    asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
-    asm volatile("mov.u32 %0, %%lanemask_lt;" : "=r"(lt_mask));
-    const bool lb4 = lane & 16, lb3 = lane & 8, lb2 = lane & 4, lb1 = lane & 2, lb0 = lane & 1;
-    // after the butterfly: even lanes hold value (lane >> 1) & 7 of Gaussian (lane >> 4); odd lanes hold the ride-along
-    // values: slot 8 + ((lane >> 2) & 3) of Gaussian (lane >> 4)
-    const bool red_lane = !lb0 || (lane & 3) == 1;
-    const int red_slot = lb0 ? 8 + ((lane >> 2) & 3) : ((lane >> 1) & 7);
-    PairSlab& slab = slabs[wslot];
-    PairSlabX& slabx = slabs_x[wslot];
-    const int sub_x0 = tile_x * kTile + (warp & 1) * kSubW;
-    const int sub_y0 = tile_y * kTile + (warp >> 1) * kSubH;
-    const int pix_x = sub_x0 + (lane & 7), pix_y = sub_y0 + (lane >> 3);
-    const bool inside = pix_x < W && pix_y < H;
-    const float pxf = (float)pix_x, pyf = (float)pix_y;
-    const float lox = (float)sub_x0, hix = (float)(sub_x0 + kSubW - 1);
-    const float loy = (float)sub_y0, hiy = (float)(sub_y0 + kSubH - 1);
-    const size_t pix_id = (size_t)pix_y * W + pix_x;
-    const size_t HW = (size_t)H * W;
-
-    const uint2 range = ranges[tile];
-
-    const float T_final = inside ? final_T[pix_id] : 0.f;
-    const uint32_t last_contributor = inside ? n_contrib[pix_id] : 0u;
-    float dp0 = 0.f, dp1 = 0.f, dp2 = 0.f;
-    if (inside) {
-        dp0 = dL_dpix[pix_id];
-        dp1 = dL_dpix[HW + pix_id];
-        dp2 = dL_dpix[2 * HW + pix_id];
-    }
-    float bg_dot_dpixel = bg[0] * dp0 + bg[1] * dp1 + bg[2] * dp2;
-    float de0 = 0.f, de1 = 0.f, de2 = 0.f;
-    if (inside) {
-        de0 = ex.dL_dout[pix_id];
-        if (ex.ch > 1) de1 = ex.dL_dout[HW + pix_id];
-        if (ex.ch > 2) de2 = ex.dL_dout[2 * HW + pix_id];
-    }
-    bg_dot_dpixel += ex.bg[0] * de0;
-    if (ex.ch > 1) bg_dot_dpixel += ex.bg[1] * de1;
-    if (ex.ch > 2) bg_dot_dpixel += ex.bg[2] * de2;
-    const float ddelx_dx = 0.5f * W, ddely_dy = 0.5f * H;
-
-    const int n = (int)__reduce_max_sync(full, last_contributor);
-    if (n == 0) return;
-
-    float T = T_final;
-    float ar0 = 0.f, ar1 = 0.f, ar2 = 0.f;      // accum_rec (advanced form, see below)
-    float ae0 = 0.f, ae1 = 0.f, ae2 = 0.f;      // same for the extra channels
-    float x0 = 0.f, x1 = 0.f, x2 = 0.f;
-    auto load_extra = [&](uint32_t id) {
-        const float* f = ex.feat + (size_t)id * ex.ch;
-        x0 = __ldg(f);
-        x1 = ex.ch > 1 ? __ldg(f + 1) : 0.f;
-        x2 = ex.ch > 2 ? __ldg(f + 2) : 0.f;
-    };
-
-    uint32_t id_cur = 0, id_next = 0;
-    float4 r0, r1, r2;
-    r0 = r1 = r2 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (lane < n) {
-        id_cur = point_list[range.x + (n - 1 - lane)];
-        const float4* p = reinterpret_cast<const float4*>(rec + id_cur);
-        r0 = __ldg(p); r1 = __ldg(p + 1); r2 = __ldg(p + 2);
-        load_extra(id_cur);
-    }
-    if (32 + lane < n) id_next = point_list[range.x + (n - 1 - 32 - lane)];
-
-    for (int base = 0; base < n; base += 32) {
-        const bool hit = (base + lane < n) && subtile_hit(lox, hix, loy, hiy, r0.x, r0.y, r0.z, r0.w, r1.x, r2.y, r2.z, r2.w);
-        const uint32_t bits = __ballot_sync(full, hit);
-        const int nhit = __popc(bits);
-        if (hit) {
-            const int slot = __popc(bits & lt_mask);
-            slab.x[slot] = r0.x; slab.y[slot] = r0.y; slab.A[slot] = r0.z; slab.B[slot] = r0.w;
-            slab.C[slot] = r1.x; slab.op[slot] = r1.y; slab.r[slot] = r1.z; slab.g[slot] = r1.w; slab.b[slot] = r2.x;
-            slab.id[slot] = id_cur;
-            slab.pos[slot] = (uint32_t)(n - 1 - base - lane);
-            slabx.e0[slot] = x0; slabx.e1[slot] = x1; slabx.e2[slot] = x2;
-        }
-        if ((nhit & 1) && lane == 0) {
-            // odd count: pad with a record that can never contribute (opacity 0, position beyond every pixel's last)
-            slab.x[nhit] = 0.f; slab.y[nhit] = 0.f; slab.A[nhit] = 0.f; slab.B[nhit] = 0.f; slab.C[nhit] = 0.f;
-            slab.op[nhit] = 0.f; slab.r[nhit] = 0.f; slab.g[nhit] = 0.f; slab.b[nhit] = 0.f;
-            slab.id[nhit] = 0u; slab.pos[nhit] = 0xffffffffu;
-            slabx.e0[nhit] = 0.f; slabx.e1[nhit] = 0.f; slabx.e2[nhit] = 0.f;
-        }
-        id_cur = id_next;
-        if (base + 32 + lane < n) {
-            const float4* p = reinterpret_cast<const float4*>(rec + id_cur);
-            r0 = __ldg(p); r1 = __ldg(p + 1); r2 = __ldg(p + 2);
-            load_extra(id_cur);
-        }
-        if (base + 64 + lane < n) id_next = point_list[range.x + (n - 1 - base - 64 - lane)];
-        __syncwarp();
-
-        for (int k = 0; k < nhit; k += 2) {
-            const P2 X = ldp(slab.x, k), Y = ldp(slab.y, k), A = ldp(slab.A, k), B = ldp(slab.B, k), Cc = ldp(slab.C, k);
-            const P2 OP = ldp(slab.op, k);
-            const uint2 POS = *reinterpret_cast<const uint2*>(slab.pos + k);
-            // power = -0.5*(A dx^2 + C dy^2) - B dx dy in the reference's op order (same as the forward kernel)
-            const P2 dx = add2(X, bc(-pxf)), dy = add2(Y, bc(-pyf));
-            const P2 q = fma2(dx, mul2(dx, A), mul2(dy, mul2(dy, Cc)));
-            const P2 u = mul2(dy, mul2(dx, B));
-            const P2 power = fma2(q, bc(-0.5f), neg2(u));
-            const P2 G = exp_pair(power);
-            const P2 og = mul2(OP, G);
-            const float al0 = fminf(0.99f, og.x), al1 = fminf(0.99f, og.y);
-            const bool act0 = (POS.x < last_contributor) && !(power.x > 0.0f) && !(al0 < 1.0f / 255.0f);
-            const bool act1 = (POS.y < last_contributor) && !(power.y > 0.0f) && !(al1 < 1.0f / 255.0f);
-            if (!__any_sync(full, act0 || act1)) continue;
-
-            const P2 Rc = ldp(slab.r, k), Gc = ldp(slab.g, k), Bc = ldp(slab.b, k);
-            // 1/(1 - alpha) for both: alpha <= 0.99 keeps the argument in [0.01, 1], so MUFU.RCP + one packed Newton
-            // step (|error| < 1 ulp) needs none of __frcp_rn's range checks
-            const P2 om = add2(bc(1.0f), neg2(p2(al0, al1)));                  // 1 - alpha
-            P2 INV;
-            {
-                float i0, i1;
-                asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(i0) : "f"(om.x));
-                asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(i1) : "f"(om.y));
-                const P2 r = p2(i0, i1);
-                INV = fma2(r, fma2(neg2(om), r, bc(1.0f)), r);
-            }
-            // ---- the recurrences chain through the two Gaussians: scalar, first 2k then 2k+1 ----
-            // accum_rec is kept in its "already advanced" form: the reference advances it with the PREVIOUS
-            // contributor's (alpha, colour) just before use (backward.cu:509-512); advancing it with the CURRENT
-            // one right after use is the same arithmetic one step earlier and needs no last_alpha / last_color
-            P2 AR0, AR1, AR2, TP, AE0, AE1, AE2;
-            AR0.x = ar0; AR1.x = ar1; AR2.x = ar2;
-            AE0.x = ae0; AE1.x = ae1; AE2.x = ae2;
-            if (act0) {
-                T = T * INV.x;
-                ar0 = al0 * Rc.x + om.x * ar0;
-                ar1 = al0 * Gc.x + om.x * ar1;
-                ar2 = al0 * Bc.x + om.x * ar2;
-                ae0 = al0 * slabx.e0[k] + om.x * ae0;
-                ae1 = al0 * slabx.e1[k] + om.x * ae1;
-                ae2 = al0 * slabx.e2[k] + om.x * ae2;
-            }
-            TP.x = T;
-            AR0.y = ar0; AR1.y = ar1; AR2.y = ar2;
-            AE0.y = ae0; AE1.y = ae1; AE2.y = ae2;
-            if (act1) {
-                T = T * INV.y;
-                ar0 = al1 * Rc.y + om.y * ar0;
-                ar1 = al1 * Gc.y + om.y * ar1;
-                ar2 = al1 * Bc.y + om.y * ar2;
-                ae0 = al1 * slabx.e0[k + 1] + om.y * ae0;
-                ae1 = al1 * slabx.e1[k + 1] + om.y * ae1;
-                ae2 = al1 * slabx.e2[k + 1] + om.y * ae2;
-            }
-            TP.y = T;
-
-            // ---- gradient algebra on the pair; a non-contributing (lane, Gaussian) is zeroed through alpha and G ----
-            const P2 al = p2(act0 ? al0 : 0.f, act1 ? al1 : 0.f);
-            const P2 Gm = p2(act0 ? G.x : 0.f, act1 ? G.y : 0.f);
-            const P2 dch = mul2(al, TP);                                       // d(channel)/d(colour)
-            P2 dLa = fma2(add2(Rc, neg2(AR0)), bc(dp0),
-                          fma2(add2(Gc, neg2(AR1)), bc(dp1), mul2(add2(Bc, neg2(AR2)), bc(dp2))));
-            const P2 F0 = ldp(slabx.e0, k), F1 = ldp(slabx.e1, k), F2 = ldp(slabx.e2, k);
-            dLa = fma2(add2(F0, neg2(AE0)), bc(de0), dLa);
-            dLa = fma2(add2(F1, neg2(AE1)), bc(de1), dLa);
-            dLa = fma2(add2(F2, neg2(AE2)), bc(de2), dLa);
-            const P2 V9 = mul2(dch, bc(de0)), V10 = mul2(dch, bc(de1)), V11 = mul2(dch, bc(de2));
-            dLa = mul2(dLa, TP);
-            dLa = fma2(mul2(bc(-T_final), INV), bc(bg_dot_dpixel), dLa);
-            const P2 dL_dG = mul2(OP, dLa);
-            const P2 gdx = mul2(Gm, dx), gdy = mul2(Gm, dy);
-            const P2 dG_ddelx = fma2(neg2(gdx), A, neg2(mul2(gdy, B)));
-            const P2 dG_ddely = fma2(neg2(gdy), Cc, neg2(mul2(gdx, B)));
-            const P2 hh = mul2(dL_dG, bc(-0.5f));
-            const P2 hx = mul2(hh, gdx), hy = mul2(hh, gdy);
-            P2 V[8];
-            V[0] = mul2(mul2(dL_dG, dG_ddelx), bc(ddelx_dx));     // dL/dmean2D.x
-            V[1] = mul2(mul2(dL_dG, dG_ddely), bc(ddely_dy));     // dL/dmean2D.y
-            V[2] = mul2(hx, dx);                                  // dL/dconic.x
-            V[3] = mul2(hx, dy);                                  // dL/dconic.y
-            V[4] = mul2(hy, dy);                                  // dL/dconic.w
-            V[5] = mul2(Gm, dLa);                                 // dL/dopacity
-            V[6] = mul2(dch, bc(dp0));                            // dL/dcolour
-            V[7] = mul2(dch, bc(dp1));
-            const P2 V8 = mul2(dch, bc(dp2));
-
-            // ---- one butterfly for both Gaussians ----
-            // bit 4: lanes 0-15 keep Gaussian 2k (.x), lanes 16-31 keep Gaussian 2k+1 (.y)
-            float w[8];
-#pragma unroll
-            for (int i = 0; i < 8; i += 2) {
-                const P2 send = p2(lb4 ? V[i].x : V[i].y, lb4 ? V[i + 1].x : V[i + 1].y);
-                const P2 keep = p2(lb4 ? V[i].y : V[i].x, lb4 ? V[i + 1].y : V[i + 1].x);
-                const P2 sum = add2(keep, p2(__shfl_xor_sync(full, send.x, 16), __shfl_xor_sync(full, send.y, 16)));
-                w[i] = sum.x; w[i + 1] = sum.y;
-            }
-            float xx[4];
-#pragma unroll
-            for (int i = 0; i < 4; i += 2) {
-                const P2 send = p2(lb3 ? w[i] : w[i + 4], lb3 ? w[i + 1] : w[i + 5]);
-                const P2 keep = p2(lb3 ? w[i + 4] : w[i], lb3 ? w[i + 5] : w[i + 1]);
-                const P2 sum = add2(keep, p2(__shfl_xor_sync(full, send.x, 8), __shfl_xor_sync(full, send.y, 8)));
-                xx[i] = sum.x; xx[i + 1] = sum.y;
-            }
-            float yy[2];
-            {
-                const P2 send = p2(lb2 ? xx[0] : xx[2], lb2 ? xx[1] : xx[3]);
-                const P2 keep = p2(lb2 ? xx[2] : xx[0], lb2 ? xx[3] : xx[1]);
-                const P2 sum = add2(keep, p2(__shfl_xor_sync(full, send.x, 4), __shfl_xor_sync(full, send.y, 4)));
-                yy[0] = sum.x; yy[1] = sum.y;
-            }
-            float z;
-            {
-                const float send = lb1 ? yy[0] : yy[1];
-                const float keep = lb1 ? yy[1] : yy[0];
-                z = keep + __shfl_xor_sync(full, send, 2);       // value 4*b3 + 2*b2 + b1 of Gaussian b4
-            }
-            // ride-along values
-            float h;
-            {
-                const P2 L[4] = {V8, V9, V10, V11};
-                float f[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float send = lb4 ? L[i].x : L[i].y;
-                    const float keep = lb4 ? L[i].y : L[i].x;
-                    f[i] = keep + __shfl_xor_sync(full, send, 16);
-                }
-                float gq[2];
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const float send = lb3 ? f[i] : f[i + 2];
-                    const float keep = lb3 ? f[i + 2] : f[i];
-                    gq[i] = keep + __shfl_xor_sync(full, send, 8);
-                }
-                {
-                    const float send = lb2 ? gq[0] : gq[1];
-                    const float keep = lb2 ? gq[1] : gq[0];
-                    h = keep + __shfl_xor_sync(full, send, 4);   // ride-along 2*b3 + b2 of Gaussian b4
-                }
-                h += __shfl_xor_sync(full, h, 2);
-            }
-            float red;
-            {
-                const float send = lb0 ? z : h;
-                const float keep = lb0 ? h : z;
-                red = keep + __shfl_xor_sync(full, send, 1);
-            }
-            if (red_lane && !(lb4 && k + 1 >= nhit)) {
-                const uint32_t gid = slab.id[k + (lb4 ? 1 : 0)];
-                atomicAdd(acc + (size_t)gid * 12 + red_slot, red);
-            }
-        }
-        __syncwarp();   // slab is rewritten by the next step
-    }
-}
-
-
 // ---- v4: transposed blocks -- lane = Gaussian for the per-pair math, lane = pixel for the recurrences --------------------
-// The pair kernel above keeps lane = pixel throughout, so every Gaussian's 9 partial gradients must be summed over the
-// warp: a third of its pair loop is the transposing butterfly (20 SHFL + 36 FSEL per two Gaussians).  Here the hits of a warp's 8x4 sub-tile are processed in blocks of 16
-// Gaussians and the work is split by what each part needs:
+// A kernel that keeps lane = pixel throughout must sum every Gaussian's 9 partial gradients over the warp: a third of
+// such a pair loop is the transposing butterfly (20 SHFL + 36 FSEL per two Gaussians; DESIGN.md §3.2).  Here the hits of
+// a warp's 8x4 sub-tile are processed in blocks of 16 Gaussians and the work is split by what each part needs:
 //   phase 1  lane = (Gaussian g, pixel half h): the lane evaluates ITS Gaussian at its 16 pixels, two pixels at a time on
 //            pair operations -- same op order as the forward (power / libdevice exp / alpha tests, bit-identical decisions) --
 //            and leaves three values per (Gaussian, pixel) in a padded shared-memory matrix: the masked opacity*G, the
@@ -331,6 +33,8 @@ render_bwd_pair_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
 //   phase 3  lane = (g, h) again: gradient algebra for its Gaussian, accumulated over its 16 pixels IN REGISTERS as five
 //            image moments of S = dL/dG * G (sum S dx, S dy, S dx^2, S dx dy, S dy^2), sum S / opacity-side and the three
 //            colour sums; no cross-lane reduction except one xor-16 add per block.  9 red.global.add per Gaussian, as before.
+// With extra channels (kExtra) c . dL/dpix becomes c . dL/dpix + e . dL/dextra throughout, K gains -T_final (bg_e .
+// dL/dextra), and phase 3 adds one sum per channel (dL/de_c, accumulator slots 9..11).
 // No shuffle and no select in the inner loops; the matrix rows are padded to 34 floats so that the 64-bit row accesses of
 // phases 1/3 (lane stride = one row) and the 32-bit column accesses of phase 2 (lane stride = one word) are both
 // bank-conflict free.
@@ -344,21 +48,26 @@ struct __align__(16) BwdWarpSmem {
     float dp0[32], dp1[32], dp2[32], K[32];     // per pixel: dL/dpixel, K = -T_final * (bg . dL/dpixel)
     uint32_t last[32];                          // per pixel: entries of the hit list up to its last contributor
 };
+struct __align__(16) BwdWarpSmemX {            // kExtra only
+    float de0[32], de1[32], de2[32];            // per pixel: dL/dextra (zero beyond ex.ch)
+};
 
 // The list a warp walks is its sub-tile's HIT LIST, written by the forward blend (render_fwd.cu): the Gaussian ids
 // that passed the sub-tile test, in tile-list order, and per pixel the number of entries up to its last contributor.
 // The backward therefore touches no instance the forward did not blend into this sub-tile: no re-test, no walk over
 // the other 7/8 of the tile list, and the per-pixel "before my last contributor" test is a compare of entry numbers.
-// 20 resident warps per SM: 96 registers, no spills (24 warps at 80 registers measured slower)
-template <int kWarps>
-__global__ void __launch_bounds__(32 * kWarps, 20 / kWarps)
+// Colour only: 20 resident warps per SM, 96 registers, no spills (24 warps at 80 registers measured slower).
+// Extra channels: 16 resident warps per SM, which leaves room for the extra registers without spills.
+template <int kWarps, bool kExtra>
+__global__ void __launch_bounds__(32 * kWarps, (kExtra ? 16 : 20) / kWarps)
 render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ sub_hits,
                       const SplatRec* __restrict__ rec, int W, int H, int tiles_x,
                       const float* __restrict__ bg, const float* __restrict__ final_T,
                       const uint32_t* __restrict__ last_entry, const float* __restrict__ dL_dpix,
-                      float* __restrict__ acc, const int32_t* __restrict__ status,
+                      float* __restrict__ acc, const int32_t* __restrict__ status, const ExtraArgs ex,
                       const uint32_t* __restrict__ tile_order) {
     __shared__ BwdWarpSmem smem[kWarps];
+    __shared__ BwdWarpSmemX smem_x[kExtra ? kWarps : 1];
     if (status[FB200_ST_OVERFLOW]) return;
 
     const unsigned full = 0xffffffffu;
@@ -370,6 +79,7 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
     int lane;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
     BwdWarpSmem& sm = smem[wslot];
+    BwdWarpSmemX& smx = smem_x[kExtra ? wslot : 0];
     const int sub_x0 = tile_x * kTile + (warp & 1) * kSubW;
     const int sub_y0 = tile_y * kTile + (warp >> 1) * kSubH;
     const uint2 range = ranges[tile];
@@ -391,7 +101,20 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
             dp1 = dL_dpix[HW + pix_id];
             dp2 = dL_dpix[2 * HW + pix_id];
         }
-        Kp = -T_final * (bg[0] * dp0 + bg[1] * dp1 + bg[2] * dp2);
+        float bg_dot = bg[0] * dp0 + bg[1] * dp1 + bg[2] * dp2;
+        if (kExtra) {
+            float de0 = 0.f, de1 = 0.f, de2 = 0.f;
+            if (inside) {
+                de0 = ex.dL_dout[pix_id];
+                if (ex.ch > 1) de1 = ex.dL_dout[HW + pix_id];
+                if (ex.ch > 2) de2 = ex.dL_dout[2 * HW + pix_id];
+            }
+            bg_dot += ex.bg[0] * de0;
+            if (ex.ch > 1) bg_dot += ex.bg[1] * de1;
+            if (ex.ch > 2) bg_dot += ex.bg[2] * de2;
+            smx.de0[lane] = de0; smx.de1[lane] = de1; smx.de2[lane] = de2;
+        }
+        Kp = -T_final * bg_dot;
         T = T_final;
         sm.dp0[lane] = dp0; sm.dp1[lane] = dp1; sm.dp2[lane] = dp2; sm.K[lane] = Kp; sm.last[lane] = le;
         top = (int)__reduce_max_sync(full, le);
@@ -420,6 +143,9 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
     const float* const pdp1 = sm.dp1 + 16 * h;
     const float* const pdp2 = sm.dp2 + 16 * h;
     const uint32_t* const plast = sm.last + 16 * h;
+    const float* const pde0 = smx.de0 + 16 * h;
+    const float* const pde1 = smx.de1 + 16 * h;
+    const float* const pde2 = smx.de2 + 16 * h;
 
     // Register prefetch, two stages deep: the Gaussian ids of block k+2 and the records of block k+1 are requested while
     // block k is processed, so neither hop of the dependent chain id -> record is waited for (without it, the id load
@@ -433,10 +159,17 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
     uint32_t nid = load_id(top), nnid = load_id(top - kBlk);
     float4 n0, n1, n2;
     n0 = n1 = n2 = make_float4(0.f, 0.f, 0.f, 0.f);
+    float nf0 = 0.f, nf1 = 0.f, nf2 = 0.f;        // extra features, prefetched with the record
     auto fetch_rec = [&](uint32_t id, int t) {    // records of the block whose top is t
         if (t - 1 - g >= 0) {
             const float4* p = reinterpret_cast<const float4*>(rec + id);
             n0 = __ldg(p); n1 = __ldg(p + 1); n2 = __ldg(p + 2);
+            if (kExtra) {
+                const float* f = ex.feat + (size_t)id * ex.ch;
+                nf0 = __ldg(f);
+                if (ex.ch > 1) nf1 = __ldg(f + 1);
+                if (ex.ch > 2) nf2 = __ldg(f + 2);
+            }
         }
     };
     fetch_rec(nid, top);
@@ -448,6 +181,7 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
         const float X = n0.x, Y = n0.y, A = n0.z, B = n0.w, Cc = n1.x;
         const float op = valid ? n1.y : 0.f;
         const float cr = valid ? n1.z : 0.f, cg = valid ? n1.w : 0.f, cb = valid ? n2.x : 0.f;
+        const float f0 = valid ? nf0 : 0.f, f1 = valid ? nf1 : 0.f, f2 = valid ? nf2 : 0.f;
         const uint32_t gid = nid;
         top -= cnt;
         nid = nnid;
@@ -485,7 +219,8 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
                 const P2 rr = p2(i0, i1);
                 inv = fma2(rr, fma2(neg2(om), rr, bc(1.0f)), rr);          // one Newton step
             }
-            const P2 cd = fma2(ldp(pdp0, k), bc(cr), fma2(ldp(pdp1, k), bc(cg), mul2(ldp(pdp2, k), bc(cb))));
+            P2 cd = fma2(ldp(pdp0, k), bc(cr), fma2(ldp(pdp1, k), bc(cg), mul2(ldp(pdp2, k), bc(cb))));
+            if (kExtra) cd = fma2(ldp(pde0, k), bc(f0), fma2(ldp(pde1, k), bc(f1), fma2(ldp(pde2, k), bc(f2), cd)));
             *reinterpret_cast<float2*>(row0 + k) = ogm;
             *reinterpret_cast<float2*>(row1 + k) = inv;
             *reinterpret_cast<float2*>(row2 + k) = mul2(am, cd);
@@ -545,6 +280,7 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
         const float rop = op > 0.f ? __frcp_rn(op) : 0.f;
         P2 sR = bc(0.f), sG = bc(0.f), sB = bc(0.f), sO = bc(0.f);
         P2 M10 = bc(0.f), M01 = bc(0.f), M20 = bc(0.f), M11 = bc(0.f), M02 = bc(0.f);
+        P2 sE0 = bc(0.f), sE1 = bc(0.f), sE2 = bc(0.f);                    // kExtra: dL/d(extra feature c)
         auto phase3 = [&](int r, int c) {
             const float dy = fadd(Y, -(py0 + (float)r));
             const int k = 8 * r + 2 * c;
@@ -553,9 +289,14 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
             const P2 d0 = ldp(pdp0, k), d1 = ldp(pdp1, k), d2 = ldp(pdp2, k);
             const P2 am = p2(fminf(0.99f, ogm.x), fminf(0.99f, ogm.y));
             const P2 Gm = mul2(ogm, bc(rop));                               // G (0 where the pair does not contribute)
-            const P2 cd = fma2(d0, bc(cr), fma2(d1, bc(cg), mul2(d2, bc(cb))));
+            P2 cd = fma2(d0, bc(cr), fma2(d1, bc(cg), mul2(d2, bc(cb))));
             const P2 dch = mul2(am, Tg);                                   // d(pixel channel)/d(colour)
             sR = fma2(dch, d0, sR); sG = fma2(dch, d1, sG); sB = fma2(dch, d2, sB);
+            if (kExtra) {
+                const P2 e0 = ldp(pde0, k), e1 = ldp(pde1, k), e2 = ldp(pde2, k);
+                cd = fma2(e0, bc(f0), fma2(e1, bc(f1), fma2(e2, bc(f2), cd)));
+                sE0 = fma2(dch, e0, sE0); sE1 = fma2(dch, e1, sE1); sE2 = fma2(dch, e2, sE2);
+            }
             const P2 dLa = fma2(Tg, cd, U);                                // dL/dalpha
             const P2 S = mul2(dLa, Gm);                                    // dL/dopacity contribution
             sO = add2(sO, S);
@@ -577,10 +318,12 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
                 phase3(sl >> 2, sl & 3);
             }
         }
-        float v[9] = {M10.x + M10.y, M01.x + M01.y, M20.x + M20.y, M11.x + M11.y, M02.x + M02.y,
-                      sO.x + sO.y, sR.x + sR.y, sG.x + sG.y, sB.x + sB.y};
+        constexpr int kSums = kExtra ? 12 : 9;
+        float v[kSums] = {M10.x + M10.y, M01.x + M01.y, M20.x + M20.y, M11.x + M11.y, M02.x + M02.y,
+                          sO.x + sO.y, sR.x + sR.y, sG.x + sG.y, sB.x + sB.y};
+        if constexpr (kExtra) { v[9] = sE0.x + sE0.y; v[10] = sE1.x + sE1.y; v[11] = sE2.x + sE2.y; }
 #pragma unroll
-        for (int i = 0; i < 9; ++i) v[i] += __shfl_xor_sync(full, v[i], 16);
+        for (int i = 0; i < kSums; ++i) v[i] += __shfl_xor_sync(full, v[i], 16);
         if (h == 0 && ((act16 >> g) & 1u)) {
             float* a = acc + (size_t)gid * 12;
             // dG/ddelx = -G (dx A + dy B), dG/ddely = -G (dy C + dx B)   (backward.cu:536-546)
@@ -590,7 +333,10 @@ render_bwd_t16_kernel(const uint2* __restrict__ ranges, const uint32_t* __restri
                       make_float4(-ddelx_dx * fmaf(A, v[0], B * v[1]), -ddely_dy * fmaf(Cc, v[1], B * v[0]),
                                   -0.5f * v[2], -0.5f * v[3]));
             atomicAdd(reinterpret_cast<float4*>(a) + 1, make_float4(-0.5f * v[4], v[5], v[6], v[7]));
-            atomicAdd(a + 8, v[8]);
+            if constexpr (kExtra)     // slots 8..11: {db, dL/dextra}, 16-byte aligned like the other two
+                atomicAdd(reinterpret_cast<float4*>(a) + 2, make_float4(v[8], v[9], v[10], v[11]));
+            else
+                atomicAdd(a + 8, v[8]);
         }
         __syncwarp();      // the matrices are rewritten by the next block
     }
@@ -607,14 +353,10 @@ cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s) {
     constexpr int kWarps = 4;   // 4-warp CTAs (half tiles): a CTA slot frees as soon as its half is done; beat 8 and 2 on C3
     const int grid = T * (kWarpsPerTile / kWarps);
     count_launch();
-    if (a.ex.ch > 0)
-        render_bwd_pair_kernel<kWarps><<<grid, 32 * kWarps, 0, s>>>(
-            a.ranges, a.point_list, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
-            a.final_T, a.n_contrib, a.dL_dpix, a.acc, a.status, a.ex, a.tile_order);
-    else
-        render_bwd_t16_kernel<kWarps><<<grid, 32 * kWarps, 0, s>>>(
-            a.ranges, a.sub_hits, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
-            a.final_T, a.last_entry, a.dL_dpix, a.acc, a.status, a.tile_order);
+    const auto kernel = a.ex.ch > 0 ? render_bwd_t16_kernel<kWarps, true> : render_bwd_t16_kernel<kWarps, false>;
+    kernel<<<grid, 32 * kWarps, 0, s>>>(
+        a.ranges, a.sub_hits, a.rec, a.prm.image_width, a.prm.image_height, a.tiles_x, a.in.d_background,
+        a.final_T, a.last_entry, a.dL_dpix, a.acc, a.status, a.ex, a.tile_order);
     return cudaGetLastError();
 }
 
