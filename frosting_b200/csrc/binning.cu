@@ -57,23 +57,12 @@ tile_scan_kernel(int T, const uint32_t* __restrict__ tile_count, uint2* __restri
         lmax = max(lmax, c);
     }
     // block exclusive scan of `local`
-    uint32_t incl = local;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t n = __shfl_up_sync(0xffffffffu, incl, o);
-        if ((tid & 31) >= o) incl += n;
-    }
+    const uint32_t incl = warp_inclusive_scan(local, tid & 31);
     if ((tid & 31) == 31) warp_sums[tid >> 5] = incl;
     __syncthreads();
     if (tid < 32) {
-        uint32_t w = warp_sums[tid];
-        uint32_t wi = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t n = __shfl_up_sync(0xffffffffu, wi, o);
-            if (tid >= o) wi += n;
-        }
-        warp_sums[tid] = wi - w;   // exclusive
+        const uint32_t w = warp_sums[tid];
+        warp_sums[tid] = warp_inclusive_scan(w, tid) - w;   // exclusive
     }
     __syncthreads();
     uint32_t run = warp_sums[tid >> 5] + incl - local;
@@ -89,23 +78,13 @@ tile_scan_kernel(int T, const uint32_t* __restrict__ tile_count, uint2* __restri
             else cls_b += 1ull << 32;
         }
     }
-    u64 inc_a = cls_a, inc_b = cls_b;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const u64 na = __shfl_up_sync(0xffffffffu, inc_a, o), nb = __shfl_up_sync(0xffffffffu, inc_b, o);
-        if ((tid & 31) >= o) { inc_a += na; inc_b += nb; }
-    }
+    const u64 inc_a = warp_inclusive_scan(cls_a, tid & 31), inc_b = warp_inclusive_scan(cls_b, tid & 31);
     __syncthreads();                 // warp_sums is reused below
     if ((tid & 31) == 31) { cls_sums[0][tid >> 5] = inc_a; cls_sums[1][tid >> 5] = inc_b; }
     __syncthreads();
     if (tid < 32) {
         const u64 wa = cls_sums[0][tid], wb = cls_sums[1][tid];
-        u64 ia = wa, ib = wb;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const u64 na = __shfl_up_sync(0xffffffffu, ia, o), nb = __shfl_up_sync(0xffffffffu, ib, o);
-            if (tid >= o) { ia += na; ib += nb; }
-        }
+        const u64 ia = warp_inclusive_scan(wa, tid), ib = warp_inclusive_scan(wb, tid);
         cls_sums[0][tid] = ia - wa;
         cls_sums[1][tid] = ib - wb;
         if (tid == 31) { cls_total[0] = ia; cls_total[1] = ib; }
@@ -206,24 +185,12 @@ scatter_kernel(int P, int tiles_x, const uint2* __restrict__ rect, const float* 
             dbits = __float_as_uint(depth[idx]);
         }
     }
-    uint32_t incl = n;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(full, incl, o);
-        if (lane >= o) incl += t;
-    }
+    const uint32_t incl = warp_inclusive_scan(n, lane);
     const uint32_t excl = incl - n;
     const uint32_t total = __shfl_sync(full, incl, 31);
     for (uint32_t base = 0; base < total; base += 32) {
         const uint32_t item = base + lane;
-        // owner = number of lanes whose inclusive count is <= item
-        int pos = 0;
-#pragma unroll
-        for (int step = 16; step >= 1; step >>= 1) {
-            const uint32_t v = __shfl_sync(full, incl, pos + step - 1);
-            if (v <= item) pos += step;
-        }
-        const int owner = min(pos, 31);
+        const int owner = warp_expand_owner(incl, item);
         const uint32_t o_excl = __shfl_sync(full, excl, owner);
         const uint32_t o_minx = __shfl_sync(full, minx, owner);
         const uint32_t o_miny = __shfl_sync(full, miny, owner);
@@ -240,13 +207,25 @@ scatter_kernel(int P, int tiles_x, const uint2* __restrict__ rect, const float* 
 }
 
 // ---- per-tile sort ----------------------------------------------------------------------------------
-// Stable LSD radix sort of one tile's keys on the 32 depth bits (4 passes of 8 bits; a pass whose digit
-// is the same for every key is skipped), followed by a fix-up that orders runs of EQUAL depth by
-// Gaussian index -- together the total order (depth_bits, idx) of the reference's stable global sort.
-// Ranking is warp-synchronous: each warp owns a contiguous slice of the list, walks it 32 keys at a
-// time and ranks equal digits with ballots (digit_peers), so no per-key shared-memory atomics are needed.
-// kShared: ping-pong buffers in shared memory (lists up to kMaxN), else in global memory (L2) with a
-// caller-provided scratch array, for lists of any length.
+// Each tile's list is sorted by the 64-bit key (depth_bits << 32 | gaussian_idx).  The keys of a tile are unique, so
+// every correct sort gives the same bits: the reference's stable order.  The shared-memory classes run the bucket sort
+// and fall back to the radix sort when a bucket is too full; the global-memory class runs the radix sort alone.  Both
+// sorts are written once for a warp (kThreads = 32, __syncwarp only) and for a CTA; t is the thread's index in it.
+template <int kThreads>
+__device__ __forceinline__ void scope_sync() {
+    if (kThreads == 32) __syncwarp(); else __syncthreads();
+}
+
+// insertion sort of b[lo, hi) on the full key
+__device__ __forceinline__ void insertion_sort(u64* b, int lo, int hi) {
+    for (int x = lo + 1; x < hi; ++x) {
+        const u64 kx = b[x];
+        int y = x - 1;
+        while (y >= lo && b[y] > kx) { b[y + 1] = b[y]; --y; }
+        b[y + 1] = kx;
+    }
+}
+
 // Lanes holding the same 8-bit digit as this lane, among the lanes with `have` set: eight ballots and eight
 // LOP3s at fixed latency.  (__match_any_sync does the same in one instruction, but its latency grows with
 // the number of distinct values -- with 32 near-random digits it dominated this kernel: ~98 k cycles per
@@ -263,24 +242,33 @@ __device__ __forceinline__ unsigned digit_peers(uint32_t d, bool have) {
     return peers;
 }
 
+// ---- radix sort -----------------------------------------------------------------------------------------------------
+// Stable LSD radix sort of one tile's keys on the 32 depth bits (4 passes of 8 bits; a pass whose digit
+// is the same for every key is skipped), followed by a fix-up that orders runs of EQUAL depth by
+// Gaussian index -- together the total order (depth_bits, idx) of the reference's stable global sort.
+// Ranking is warp-synchronous: each warp owns a contiguous slice of the list, walks it 32 keys at a
+// time and ranks equal digits with ballots (digit_peers), so no per-key shared-memory atomics are needed.
+// Sorts src[0, n) with dst as the other ping-pong buffer, both in shared memory or, for lists of any length, in global
+// memory (L2); returns the buffer holding the result.
+// counters: (kThreads / 32) * 256 words, one digit histogram per warp; s_misc: 1 + min(kThreads, 256) / 32 words.
 template <int kThreads>
 // NOTE: no __restrict__ on any of these pointers -- they are written by other threads of the CTA and
 // re-read after barriers; with __restrict__ nvcc forwards a thread's own stale store across
 // __syncthreads() (observed: s_misc[0] kept in a register, threads disagreeing on `skip`, deadlock).
-__device__ __forceinline__ void radix_sort_tile(u64* a, u64* b, int n,
-                                                uint32_t* counters /* [kThreads/32][256] */,
-                                                volatile uint32_t* s_misc, u64*& result) {
+__device__ __forceinline__ u64* radix_sort(u64* src, u64* dst, int n, uint32_t* counters, volatile uint32_t* s_misc,
+                                           int t) {
     constexpr int kWarps = kThreads / 32;
-    const unsigned full = 0xffffffffu;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // contiguous slice per warp, multiple of 32
+    constexpr int kOwners = kThreads < 256 ? kThreads : 256;    // step 2: thread t < kOwners owns kPer digits
+    constexpr int kPer = 256 / kOwners;
+    const int warp = t >> 5, lane = t & 31;
+    // contiguous slice per warp, multiple of 32; the whole list at warp scope, spelled out (with the general bounds,
+    // ptxas re-reads the shared-memory window base for every key of the tiny kernel's bucket insertion loop)
     const int seg = (((n + kWarps - 1) / kWarps) + 31) & ~31;
-    const int seg_lo = min(n, warp * seg), seg_hi = min(n, seg_lo + seg);
-    u64* src = a;
-    u64* dst = b;
+    const int seg_lo = kWarps == 1 ? 0 : min(n, warp * seg), seg_hi = kWarps == 1 ? n : min(n, seg_lo + seg);
     for (int shift = 32; shift < 64; shift += 8) {
-        for (int i = tid; i < kWarps * 256; i += kThreads) counters[i] = 0;
-        __syncthreads();
+        for (int i = t; i < kWarps * 256; i += kThreads) counters[i] = 0;
+        if (t == 0) s_misc[0] = 0;
+        scope_sync<kThreads>();
         // 1. per-warp digit histogram of its slice
         for (int i0 = seg_lo; i0 < seg_hi; i0 += 32) {
             const int i = i0 + lane;
@@ -290,41 +278,43 @@ __device__ __forceinline__ void radix_sort_tile(u64* a, u64* b, int n,
             if (have && (__ffs(peers) - 1) == lane) counters[warp * 256 + d] += __popc(peers);
             __syncwarp();
         }
-        __syncthreads();
+        scope_sync<kThreads>();
         // 2. digit totals, uniform-digit test, exclusive offsets per (digit, warp)
-        if (tid == 0) s_misc[0] = 0;
-        __syncthreads();
         uint32_t tot = 0;
-        if (tid < 256) {
+        if (t < kOwners) {
 #pragma unroll
-            for (int w = 0; w < kWarps; ++w) tot += counters[w * 256 + tid];
-            if (tot == (uint32_t)n) s_misc[0] = 1;   // every key has this digit: pass is the identity
+            for (int k = 0; k < kPer; ++k) {
+                uint32_t c = 0;
+#pragma unroll
+                for (int w = 0; w < kWarps; ++w) c += counters[w * 256 + kPer * t + k];
+                if (c == (uint32_t)n) s_misc[0] = 1;   // every key has this digit: pass is the identity
+                tot += c;
+            }
         }
-        __syncthreads();
+        scope_sync<kThreads>();
         const bool skip = s_misc[0] != 0;
         if (!skip) {
-            // block exclusive scan of tot over the 256 digits (threads 0..255 = 8 warps)
-            uint32_t incl = tot;
-            if (tid < 256) {
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const uint32_t t = __shfl_up_sync(full, incl, o);
-                    if (lane >= o) incl += t;
-                }
+            // exclusive scan of tot over the owners
+            uint32_t incl = 0;
+            if (t < kOwners) {
+                incl = warp_inclusive_scan(tot, lane);
                 if (lane == 31) s_misc[1 + warp] = incl;
             }
-            __syncthreads();
-            if (tid < 256) {
+            scope_sync<kThreads>();
+            if (t < kOwners) {
                 uint32_t base = incl - tot;
                 for (int w = 0; w < warp; ++w) base += s_misc[1 + w];
 #pragma unroll
-                for (int w = 0; w < kWarps; ++w) {
-                    const uint32_t c = counters[w * 256 + tid];
-                    counters[w * 256 + tid] = base;
-                    base += c;
+                for (int k = 0; k < kPer; ++k) {
+#pragma unroll
+                    for (int w = 0; w < kWarps; ++w) {
+                        const uint32_t c = counters[w * 256 + kPer * t + k];
+                        counters[w * 256 + kPer * t + k] = base;
+                        base += c;
+                    }
                 }
             }
-            __syncthreads();
+            scope_sync<kThreads>();
             // 3. stable scatter
             for (int i0 = seg_lo; i0 < seg_hi; i0 += 32) {
                 const int i = i0 + lane;
@@ -341,110 +331,26 @@ __device__ __forceinline__ void radix_sort_tile(u64* a, u64* b, int n,
                 }
                 __syncwarp();
             }
-            u64* t = src; src = dst; dst = t;
+            u64* tmp = src; src = dst; dst = tmp;
         }
-        __syncthreads();
+        scope_sync<kThreads>();
     }
     // 4. order runs of equal depth by Gaussian index (rare: exact float ties)
-    for (int i = tid; i < n; i += kThreads) {
+    for (int i = t; i < n; i += kThreads) {
         const uint32_t d = (uint32_t)(src[i] >> 32);
         const bool run_start = (i == 0 || (uint32_t)(src[i - 1] >> 32) != d) && (i + 1 < n) &&
                                (uint32_t)(src[i + 1] >> 32) == d;
         if (run_start) {
             int e = i + 1;
             while (e < n && (uint32_t)(src[e] >> 32) == d) ++e;
-            for (int x = i + 1; x < e; ++x) {          // insertion sort of the run [i, e)
-                const u64 kx = src[x];
-                int y = x - 1;
-                while (y >= i && src[y] > kx) { src[y + 1] = src[y]; --y; }
-                src[y + 1] = kx;
-            }
+            insertion_sort(src, i, e);
         }
     }
-    __syncthreads();
-    result = src;
-}
-
-// Stable LSD radix sort of one tile's keys by ONE warp (the fallback of the bucket sort below; round 1's sort of the
-// tiny class): same ranking as radix_sort_tile, __syncwarp only.  Returns the buffer holding the result.
-__device__ __forceinline__ u64* radix_sort_warp(u64* src, u64* dst, int n, uint32_t* cnt, int lane) {
-    const unsigned full = 0xffffffffu;
-    for (int shift = 32; shift < 64; shift += 8) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) cnt[lane + 32 * k] = 0;
-        __syncwarp();
-        // 1. digit histogram
-        for (int i0 = 0; i0 < n; i0 += 32) {
-            const int i = i0 + lane;
-            const bool have = i < n;
-            const uint32_t d = have ? (uint32_t)(src[i] >> shift) & 0xffu : 0u;
-            const unsigned peers = digit_peers(d, have);
-            if (have && (__ffs(peers) - 1) == lane) cnt[d] += __popc(peers);
-            __syncwarp();
-        }
-        // 2. exclusive offsets: lane l owns digits 8l .. 8l+7; a digit shared by every key makes the pass an identity
-        uint32_t c[8];
-        uint32_t tot = 0;
-        bool uniform = false;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            c[k] = cnt[8 * lane + k];
-            uniform |= c[k] == (uint32_t)n;
-            tot += c[k];
-        }
-        if (__any_sync(full, uniform)) continue;
-        uint32_t incl = tot;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(full, incl, o);
-            if (lane >= o) incl += t;
-        }
-        uint32_t base = incl - tot;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            cnt[8 * lane + k] = base;
-            base += c[k];
-        }
-        __syncwarp();
-        // 3. stable scatter, 32 keys at a time in list order
-        for (int i0 = 0; i0 < n; i0 += 32) {
-            const int i = i0 + lane;
-            const bool have = i < n;
-            const u64 k = have ? src[i] : 0ull;
-            const uint32_t d = have ? (uint32_t)(k >> shift) & 0xffu : 0u;
-            const unsigned peers = digit_peers(d, have);
-            uint32_t off = 0;
-            if (have) off = cnt[d] + __popc(peers & ((1u << lane) - 1u));
-            __syncwarp();
-            if (have) {
-                dst[off] = k;
-                if ((__ffs(peers) - 1) == lane) cnt[d] += __popc(peers);
-            }
-            __syncwarp();
-        }
-        u64* t = src; src = dst; dst = t;
-    }
-    // 4. order runs of equal depth by Gaussian index (rare: exact float ties)
-    for (int i = lane; i < n; i += 32) {
-        const uint32_t d = (uint32_t)(src[i] >> 32);
-        const bool run_start = (i == 0 || (uint32_t)(src[i - 1] >> 32) != d) && (i + 1 < n) &&
-                               (uint32_t)(src[i + 1] >> 32) == d;
-        if (run_start) {
-            int e = i + 1;
-            while (e < n && (uint32_t)(src[e] >> 32) == d) ++e;
-            for (int x = i + 1; x < e; ++x) {          // insertion sort of the run [i, e)
-                const u64 kx = src[x];
-                int y = x - 1;
-                while (y >= i && src[y] > kx) { src[y + 1] = src[y]; --y; }
-                src[y + 1] = kx;
-            }
-        }
-    }
-    __syncwarp();
+    scope_sync<kThreads>();
     return src;
 }
 
-// ---- bucket sort: the common case of every class --------------------------------------------------------------------
+// ---- bucket sort: the common case of every shared-memory class ------------------------------------------------------
 // A tile's depths are a few hundred to a few thousand floats inside one narrow interval, close to uniform in it.  Instead
 // of four 8-bit LSD passes (two ballot-ranked sweeps each: ~10 warp-instructions per key), the
 // keys are dropped into kBuckets >= n equal-width buckets over the tile's own [min, max] of depth bits -- one histogram
@@ -454,13 +360,8 @@ __device__ __forceinline__ u64* radix_sort_warp(u64* src, u64* dst, int n, uint3
 // sort instead, decided per tile on the device.
 constexpr int kInsertMax = 24;
 
-template <int kThreads>
-__device__ __forceinline__ void scope_sync() {
-    if (kThreads == 32) __syncwarp(); else __syncthreads();
-}
-
 // Sorts a[0, n) into b[0, n); returns false (uniformly, b unspecified, a intact) when a bucket is too full.
-// cnt: kBuckets words; s_misc: words {min, max, maxcnt}; warp_tot: 32 words (CTA scope only); t: thread index in the scope.
+// cnt: kBuckets words; s_misc: words {min, max, maxcnt}; warp_tot: 32 words (CTA scope only).
 template <int kThreads, int kBuckets>
 __device__ __forceinline__ bool bucket_sort_tile(const u64* a, u64* b, int n, uint32_t* cnt, uint32_t* s_misc,
                                                  uint32_t* warp_tot, int t) {
@@ -493,12 +394,7 @@ __device__ __forceinline__ bool bucket_sort_tile(const u64* a, u64* b, int n, ui
         const uint32_t c = cnt[t * kPer + k];
         local += c; lmaxc = max(lmaxc, c);
     }
-    uint32_t incl = local;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t v = __shfl_up_sync(full, incl, o);
-        if ((t & 31) >= o) incl += v;
-    }
+    const uint32_t incl = warp_inclusive_scan(local, t & 31);
     lmaxc = __reduce_max_sync(full, lmaxc);
     uint32_t warp_base = 0;
     if (kThreads > 32) {
@@ -524,17 +420,34 @@ __device__ __forceinline__ bool bucket_sort_tile(const u64* a, u64* b, int n, ui
     }
     scope_sync<kThreads>();
     // 4. insertion sort inside each bucket; cnt[j] is now the END of bucket j
-    for (int j = t; j < kBuckets; j += kThreads) {
-        const int lo = j ? (int)cnt[j - 1] : 0, hi = (int)cnt[j];
-        for (int x = lo + 1; x < hi; ++x) {
-            const u64 kx = b[x];
-            int y = x - 1;
-            while (y >= lo && b[y] > kx) { b[y + 1] = b[y]; --y; }
-            b[y + 1] = kx;
-        }
-    }
+    for (int j = t; j < kBuckets; j += kThreads) insertion_sort(b, j ? (int)cnt[j - 1] : 0, (int)cnt[j]);
     scope_sync<kThreads>();
     return true;
+}
+
+// Sorts the keys of the tile with range rg in shared memory -- the bucket sort, else the radix sort -- and writes them
+// back, with their Gaussian indices to point_list.  buf_a, buf_b: kMaxN keys each; counters: kMaxN bucket words, whose
+// first (kThreads / 32) * 256 double as the radix sort's per-warp digit counters; s_misc: 3 words at warp scope, 9 at
+// CTA scope; warp_tot: 32 words (CTA scope only).
+template <int kThreads, int kMaxN>
+__device__ __forceinline__ void sort_tile_shared(u64* keys, uint32_t* point_list, uint2 rg, u64* buf_a, u64* buf_b,
+                                                 uint32_t* counters, uint32_t* s_misc, uint32_t* warp_tot, int t) {
+    static_assert(kMaxN >= (kThreads / 32) * 256, "counter aliasing");
+    const int n = (int)(rg.y - rg.x);
+    u64* g = keys + rg.x;
+    for (int i = t; i < n; i += kThreads) buf_a[i] = g[i];
+    scope_sync<kThreads>();
+    const u64* res = buf_b;
+    if (!bucket_sort_tile<kThreads, kMaxN>(buf_a, buf_b, n, counters, s_misc, warp_tot, t)) {
+        scope_sync<kThreads>();
+        res = radix_sort<kThreads>(buf_a, buf_b, n, counters, s_misc, t);
+    }
+    for (int i = t; i < n; i += kThreads) {
+        const u64 k = res[i];
+        g[i] = k;
+        point_list[rg.x + i] = (uint32_t)k;
+    }
+    scope_sync<kThreads>();
 }
 
 template <int kThreads, int kMaxN, bool kDynamic>
@@ -542,9 +455,6 @@ __global__ void __launch_bounds__(kThreads)
 tile_sort_shared_kernel(const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list,
                         const uint2* __restrict__ ranges, u64* __restrict__ keys,
                         uint32_t* __restrict__ point_list, const int32_t* __restrict__ status) {
-    // counters: kMaxN bucket words for the bucket sort; their first (kThreads / 32) * 256 double as the radix fallback's
-    // per-warp digit counters
-    static_assert(kMaxN >= (kThreads / 32) * 256, "counter aliasing");
     extern __shared__ __align__(16) unsigned char dyn_smem[];
     __shared__ u64 stat_a[kDynamic ? 1 : kMaxN];
     __shared__ u64 stat_b[kDynamic ? 1 : kMaxN];
@@ -556,24 +466,9 @@ tile_sort_shared_kernel(const uint32_t* __restrict__ list, const uint32_t* __res
     uint32_t* counters = kDynamic ? reinterpret_cast<uint32_t*>(dyn_smem + 2 * sizeof(u64) * kMaxN) : stat_counters;
     if (status[FB200_ST_OVERFLOW]) return;
     const uint32_t count = *n_list;
-    for (uint32_t w = blockIdx.x; w < count; w += gridDim.x) {
-        const uint2 rg = ranges[list[w]];
-        const int n = (int)(rg.y - rg.x);
-        u64* g = keys + rg.x;
-        for (int i = threadIdx.x; i < n; i += kThreads) buf_a[i] = g[i];
-        __syncthreads();
-        u64* res = buf_b;
-        if (!bucket_sort_tile<kThreads, kMaxN>(buf_a, buf_b, n, counters, s_misc, s_warp_tot, threadIdx.x)) {
-            __syncthreads();
-            radix_sort_tile<kThreads>(buf_a, buf_b, n, counters, s_misc, res);
-        }
-        for (int i = threadIdx.x; i < n; i += kThreads) {
-            const u64 k = res[i];
-            g[i] = k;
-            point_list[rg.x + i] = (uint32_t)k;
-        }
-        __syncthreads();
-    }
+    for (uint32_t w = blockIdx.x; w < count; w += gridDim.x)
+        sort_tile_shared<kThreads, kMaxN>(keys, point_list, ranges[list[w]], buf_a, buf_b, counters, s_misc, s_warp_tot,
+                                          threadIdx.x);
 }
 
 // ---- tiny lists: one WARP per tile ---------------------------------------------------------------------
@@ -600,23 +495,12 @@ tile_sort_warp_kernel(const uint32_t* __restrict__ list, const uint32_t* __restr
             if (lane == 0) point_list[rg.x] = (uint32_t)g[0];
             continue;
         }
-        u64* src = s_a[warp];
-        u64* dst = s_b[warp];
-        for (int i = lane; i < n; i += 32) src[i] = g[i];
-        __syncwarp();
-        const u64* res = dst;
-        if (!bucket_sort_tile<32, kSortTinyMax>(src, dst, n, s_cnt[warp], s_misc[warp], nullptr, lane))
-            res = radix_sort_warp(src, dst, n, s_cnt[warp], lane);
-        for (int i = lane; i < n; i += 32) {
-            const u64 k = res[i];
-            g[i] = k;
-            point_list[rg.x + i] = (uint32_t)k;
-        }
-        __syncwarp();
+        sort_tile_shared<32, kSortTinyMax>(keys, point_list, rg, s_a[warp], s_b[warp], s_cnt[warp], s_misc[warp], nullptr,
+                                           lane);
     }
 }
 
-// Lists longer than the shared-memory class: same algorithm, ping-pong between the key array and a
+// Lists longer than the shared-memory classes: the radix sort alone, ping-pong between the key array and a
 // scratch array in global memory (L2-resident for any realistic tile).
 template <int kThreads>
 __global__ void __launch_bounds__(kThreads)
@@ -631,8 +515,7 @@ tile_sort_global_kernel(const uint32_t* __restrict__ list, const uint32_t* __res
         const uint2 rg = ranges[list[w]];
         const int n = (int)(rg.y - rg.x);
         u64* g = keys + rg.x;
-        u64* res;
-        radix_sort_tile<kThreads>(g, scratch + rg.x, n, counters, s_misc, res);
+        const u64* res = radix_sort<kThreads>(g, scratch + rg.x, n, counters, s_misc, threadIdx.x);
         for (int i = threadIdx.x; i < n; i += kThreads) {
             const u64 k = res[i];
             if (res != g) g[i] = k;

@@ -226,7 +226,7 @@ constexpr int kPreSpan = kPreThreads * kPreRounds;     // Gaussians per CTA
 // ---- per-tile instance counts for the 32 rectangles of a warp, warp-balanced ----
 // The reference's duplicateWithKeys walks each splat's tile rectangle in a serial per-thread double loop
 // (rasterizer_impl.cu:98-108) and so did round 1's counting here: one 12x12-tile splat kept its warp busy for 144
-// dependent iterations.  Same expansion as scatter_kernel (binning.cu): the warp scans its
+// dependent iterations.  Same expansion as scatter_kernel (binning.cu, warp_expand_owner): the warp scans its
 // 32 rectangle sizes and walks the concatenated instance list 32 instances per step.
 __device__ __forceinline__ void count_tiles(const FwdArgs& a, uint2 rect, int idx, int lane) {
     const unsigned full = 0xffffffffu;
@@ -247,24 +247,13 @@ __device__ __forceinline__ void count_tiles(const FwdArgs& a, uint2 rect, int id
             for (uint32_t ty = miny; ty < maxy; ++ty)
                 for (uint32_t tx = minx; tx < maxx; ++tx) atomicAdd(a.tile_count + ty * gxw + tx, 1u);
     } else {
-        uint32_t incl = cnt;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(full, incl, o);
-            if (lane >= o) incl += t;
-        }
+        const uint32_t incl = warp_inclusive_scan(cnt, lane);
         const uint32_t excl = incl - cnt;
         const uint32_t total = __shfl_sync(full, incl, 31);
         const float rw = w ? __frcp_rn((float)w) : 0.f;
         for (uint32_t base = 0; base < total; base += 32) {
             const uint32_t item = base + lane;
-            int pos = 0;                      // owner = number of lanes whose inclusive count is <= item
-#pragma unroll
-            for (int step = 16; step >= 1; step >>= 1) {
-                const uint32_t t = __shfl_sync(full, incl, pos + step - 1);
-                if (t <= item) pos += step;
-            }
-            const int owner = min(pos, 31);
+            const int owner = warp_expand_owner(incl, item);
             const uint32_t o_excl = __shfl_sync(full, excl, owner);
             const uint32_t o_min = __shfl_sync(full, rect.x, owner);
             const uint32_t o_w = __shfl_sync(full, w, owner);
