@@ -20,7 +20,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", ARCH, "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr",
-] + os.environ.get("FB200_NVCC_DEFS", "").split()      # A/B builds only, e.g. "-DFB200_PRE_CTAS=3"
+]
 
 
 def _deps_mtime():

@@ -23,14 +23,6 @@ namespace fb200 {
 
 namespace {
 
-__device__ constexpr float kC0 = 0.28209479177387814f;
-__device__ constexpr float kC1 = 0.4886025119029199f;
-__device__ constexpr float kC2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                                     -1.0925484305920792f, 0.5462742152960396f};
-__device__ constexpr float kC3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                                     0.3731763325901154f, -0.4570457994644658f, 1.445305721320277f,
-                                     -0.5900435899266435f};
-
 struct V3 { float x, y, z; };
 __device__ __forceinline__ V3 v3(float x, float y, float z) { V3 r; r.x = x; r.y = y; r.z = z; return r; }
 __device__ __forceinline__ float dot(V3 a, V3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
@@ -64,35 +56,17 @@ __device__ __forceinline__ void zero_warp_rows(const BwdArgs& a, size_t g, int M
         for (int k = lane; k < M * 3 * 32; k += 32) a.g.d_dL_dsh[(size_t)M * 3 * g + k] = 0.f;
 }
 
-// zero gradient row of ONE Gaussian
-__device__ __forceinline__ void zero_row(const BwdArgs& a, size_t i, int M) {
-    for (int k = 0; k < 3; ++k) {
-        a.g.d_dL_dmeans2D[3 * i + k] = 0.f; a.g.d_dL_dmeans3D[3 * i + k] = 0.f;
-        if (a.g.d_dL_dcolors) a.g.d_dL_dcolors[3 * i + k] = 0.f;
-        if (a.g.d_dL_dscales) a.g.d_dL_dscales[3 * i + k] = 0.f;
-    }
-    a.g.d_dL_dopacity[i] = 0.f;
-    if (a.g.d_dL_dcov3D) for (int k = 0; k < 6; ++k) a.g.d_dL_dcov3D[6 * i + k] = 0.f;
-    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (a.g.d_dL_drotations) reinterpret_cast<float4*>(a.g.d_dL_drotations)[i] = z4;
-    if (a.g.d_dL_dsh != nullptr && M == 16) {
-        float4* p = reinterpret_cast<float4*>(a.g.d_dL_dsh + 48 * i);
-#pragma unroll
-        for (int k = 0; k < 12; ++k) p[k] = z4;
-    } else if (a.g.d_dL_dsh != nullptr) {
-        for (int k = 0; k < 3 * M; ++k) a.g.d_dL_dsh[(size_t)M * 3 * i + k] = 0.f;
-    }
-}
-
 // ---- one row per lane <-> shared staging block, moved by the whole warp ----
 // A lane reading ITS row straight from global memory (12 x 128-bit at a 192-byte stride, or 45 scalars at 180 bytes
 // for Frosting's `rest` rows) costs 32 LSU wavefronts per instruction -- two to seven times the sectors the rows
 // occupy -- and that, not arithmetic, bounded this kernel.  Here the warp walks the rows together: each instruction
-// touches one or two rows contiguously (<= 12 sectors); the lanes then work on their rows in shared memory (row stride
-// odd in words / 13 in float4: conflict-free).  `rows` <= 32 rows are live; lane r holds row r's pointer.
-constexpr int kStageStride4 = 13;                    // float4 per staged row (12 used) -- standard path, M == 16
+// touches one or two rows contiguously (<= 12 sectors); the lanes then work on their rows in shared memory.  Every SH
+// row -- M == 16, any other width, Frosting's dc | rest -- is staged in one layout: coefficient-major, RGB innermost, at
+// most 48 floats, 13 float4 apart so that the lanes' per-row LDS.128 / STS.128 are conflict-free (the scalar movers
+// write one row per instruction, lane = float: their banks do not depend on the stride).  `rows` <= 32 rows are live;
+// lane r holds row r's pointer.
+constexpr int kStageStride4 = 13;                    // float4 per staged row (12 used)
 constexpr int kStageStride = 4 * kStageStride4;      // floats per staged row: 52
-constexpr int kFrostStride = 49;                     // frosting path: 3 dc + 45 rest floats, odd stride
 
 // The loads of a batch are all issued before the first one is consumed (a plain loop would pay one memory round trip
 // per row: load -> store to shared -> next load).
@@ -170,11 +144,13 @@ __device__ __forceinline__ void warp_gather_rows(const float* my_row, int nf, fl
     __syncwarp();
 }
 
-__device__ __forceinline__ void warp_scatter_rows(float* my_row, int nf, const float* stage, int stride, int rows, int lane) {
+// rows of nf floats of which the first n_staged are staged: the others go out as zeros
+__device__ __forceinline__ void warp_scatter_rows(float* my_row, int nf, int n_staged, const float* stage, int stride,
+                                                  int rows, int lane) {
     __syncwarp();
     for (int r = 0; r < rows; ++r) {
         float* p = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, (unsigned long long)my_row, r));
-        for (int k = lane; k < nf; k += 32) p[k] = stage[r * stride + k];
+        for (int k = lane; k < nf; k += 32) p[k] = k < n_staged ? stage[r * stride + k] : 0.f;
     }
     __syncwarp();
 }
@@ -224,10 +200,10 @@ geom_bwd_kernel(BwdArgs a) {
         } else {
             idx = jb + (in_rows ? lane : 0);
             active = in_rows && a.radii[idx] > 0;
-            if (!__any_sync(full, active)) {
-                // nothing rendered in this run (the common case under occlusion culling): zeros, coalesced
-                if (rows == 32) zero_warp_rows(a, (size_t)jb, M, lane);
-                else if (in_rows) zero_row(a, (size_t)idx, M);
+            if (rows == 32 && !__any_sync(full, active)) {
+                // nothing rendered in this run (the common case under occlusion culling): zeros, coalesced.  The final,
+                // shorter run goes through the compute path below, whose unrendered lanes store zeros.
+                zero_warp_rows(a, (size_t)jb, M, lane);
                 continue;
             }
         }
@@ -236,7 +212,6 @@ geom_bwd_kernel(BwdArgs a) {
 
         float* dsh = (!kFrost && a.g.d_dL_dsh != nullptr && M > 0) ? a.g.d_dL_dsh + i * M * 3 : nullptr;
         const bool has_sh = kFrost || (a.in.d_shs != nullptr && M > 0 && dsh != nullptr);
-        const bool staged4 = !kFrost && has_sh && M == 16;
         // the rows every lane reads for itself further down: start them moving now, beside the staged SH rows
         auto touch = [](const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); };
         touch(a.acc + i * 12);
@@ -249,13 +224,16 @@ geom_bwd_kernel(BwdArgs a) {
         }
         if (kFrost) {
             // dc | rest rows into the staging block: [0..2] dc, [3..] rest
-            warp_gather_rows(fr.d_sh_rest + i * (size_t)fr.sh_rest * 3, fr.sh_rest * 3, stage + 3, kFrostStride, rows, lane);
-            stage[lane * kFrostStride + 0] = __ldg(fr.d_sh_dc + 3 * i);
-            stage[lane * kFrostStride + 1] = __ldg(fr.d_sh_dc + 3 * i + 1);
-            stage[lane * kFrostStride + 2] = __ldg(fr.d_sh_dc + 3 * i + 2);
-        } else if (staged4) {
+            warp_gather_rows(fr.d_sh_rest + i * (size_t)fr.sh_rest * 3, fr.sh_rest * 3, stage + 3, kStageStride, rows, lane);
+            stage[lane * kStageStride + 0] = __ldg(fr.d_sh_dc + 3 * i);
+            stage[lane * kStageStride + 1] = __ldg(fr.d_sh_dc + 3 * i + 1);
+            stage[lane * kStageStride + 2] = __ldg(fr.d_sh_dc + 3 * i + 2);
+        } else if (has_sh && M == 16) {
             if (!kList && rows == 32) warp_gather_block4(a.in.d_shs + (size_t)jb * 48, stage4, lane);
             else warp_gather_rows4(a.in.d_shs + i * 48, stage4, rows, lane);
+        } else if (has_sh) {
+            // coefficients beyond degree 3 (M > 16) are not read: their gradients are zero
+            warp_gather_rows(a.in.d_shs + i * M * 3, min(3 * M, 48), stage, kStageStride, rows, lane);
         }
 
         float g_mean2d_x, g_mean2d_y, g_op;
@@ -386,82 +364,43 @@ geom_bwd_kernel(BwdArgs a) {
                 bv[3] = -kC1 * x; bx[3] = -kC1;
                 if (D > 1) {
                     const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                    bv[4] = kC2[0] * xy;                 bx[4] = kC2[0] * y;        by[4] = kC2[0] * x;
-                    bv[5] = kC2[1] * yz;                 by[5] = kC2[1] * z;        bz[5] = kC2[1] * y;
-                    bv[6] = kC2[2] * (2.f * zz - xx - yy); bx[6] = kC2[2] * 2.f * -x; by[6] = kC2[2] * 2.f * -y; bz[6] = kC2[2] * 4.f * z;
-                    bv[7] = kC2[3] * xz;                 bx[7] = kC2[3] * z;        bz[7] = kC2[3] * x;
-                    bv[8] = kC2[4] * (xx - yy);          bx[8] = kC2[4] * 2.f * x;  by[8] = kC2[4] * 2.f * -y;
+                    bv[4] = kC2_0 * xy;                 bx[4] = kC2_0 * y;        by[4] = kC2_0 * x;
+                    bv[5] = kC2_1 * yz;                 by[5] = kC2_1 * z;        bz[5] = kC2_1 * y;
+                    bv[6] = kC2_2 * (2.f * zz - xx - yy); bx[6] = kC2_2 * 2.f * -x; by[6] = kC2_2 * 2.f * -y; bz[6] = kC2_2 * 4.f * z;
+                    bv[7] = kC2_3 * xz;                 bx[7] = kC2_3 * z;        bz[7] = kC2_3 * x;
+                    bv[8] = kC2_4 * (xx - yy);          bx[8] = kC2_4 * 2.f * x;  by[8] = kC2_4 * 2.f * -y;
                     if (D > 2) {
-                        bv[9] = kC3[0] * y * (3.f * xx - yy);            bx[9] = kC3[0] * 6.f * xy;  by[9] = kC3[0] * 3.f * (xx - yy);
-                        bv[10] = kC3[1] * xy * z;                        bx[10] = kC3[1] * yz;      by[10] = kC3[1] * xz;   bz[10] = kC3[1] * xy;
-                        bv[11] = kC3[2] * y * (4.f * zz - xx - yy);      bx[11] = kC3[2] * -2.f * xy; by[11] = kC3[2] * (-3.f * yy + 4.f * zz - xx); bz[11] = kC3[2] * 8.f * yz;
-                        bv[12] = kC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy); bx[12] = kC3[3] * -6.f * xz; by[12] = kC3[3] * -6.f * yz; bz[12] = kC3[3] * 3.f * (2.f * zz - xx - yy);
-                        bv[13] = kC3[4] * x * (4.f * zz - xx - yy);      bx[13] = kC3[4] * (-3.f * xx + 4.f * zz - yy); by[13] = kC3[4] * -2.f * xy; bz[13] = kC3[4] * 8.f * xz;
-                        bv[14] = kC3[5] * z * (xx - yy);                 bx[14] = kC3[5] * 2.f * xz; by[14] = kC3[5] * -2.f * yz; bz[14] = kC3[5] * (xx - yy);
-                        bv[15] = kC3[6] * x * (xx - 3.f * yy);           bx[15] = kC3[6] * 3.f * (xx - yy); by[15] = kC3[6] * -6.f * xy;
+                        bv[9] = kC3_0 * y * (3.f * xx - yy);            bx[9] = kC3_0 * 6.f * xy;  by[9] = kC3_0 * 3.f * (xx - yy);
+                        bv[10] = kC3_1 * xy * z;                        bx[10] = kC3_1 * yz;      by[10] = kC3_1 * xz;   bz[10] = kC3_1 * xy;
+                        bv[11] = kC3_2 * y * (4.f * zz - xx - yy);      bx[11] = kC3_2 * -2.f * xy; by[11] = kC3_2 * (-3.f * yy + 4.f * zz - xx); bz[11] = kC3_2 * 8.f * yz;
+                        bv[12] = kC3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy); bx[12] = kC3_3 * -6.f * xz; by[12] = kC3_3 * -6.f * yz; bz[12] = kC3_3 * 3.f * (2.f * zz - xx - yy);
+                        bv[13] = kC3_4 * x * (4.f * zz - xx - yy);      bx[13] = kC3_4 * (-3.f * xx + 4.f * zz - yy); by[13] = kC3_4 * -2.f * xy; bz[13] = kC3_4 * 8.f * xz;
+                        bv[14] = kC3_5 * z * (xx - yy);                 bx[14] = kC3_5 * 2.f * xz; by[14] = kC3_5 * -2.f * yz; bz[14] = kC3_5 * (xx - yy);
+                        bv[15] = kC3_6 * x * (xx - 3.f * yy);           bx[15] = kC3_6 * 3.f * (xx - yy); by[15] = kC3_6 * -6.f * xy;
                     }
                 }
             }
             const int ncoef = (D + 1) * (D + 1);
             const float dR[3] = {dRGB.x, dRGB.y, dRGB.z};
             float ax[3] = {0.f, 0.f, 0.f}, ay[3] = {0.f, 0.f, 0.f}, az[3] = {0.f, 0.f, 0.f};
-            if (kFrost) {
-                // dc | rest values from the staging block; their gradients overwrite them there
-                float* srow = stage + lane * kFrostStride;
+            // the staged row's values; their gradients overwrite them there (zeros past the degree's coefficients)
+            float4* srow4 = stage4 + lane * kStageStride4;
 #pragma unroll
-                for (int k = 0; k < 16; ++k) {
-                    if (k < M) {
+            for (int q = 0; q < 12; ++q) {
+                float o[4] = {0.f, 0.f, 0.f, 0.f};
+                if (4 * q < 3 * ncoef) {
+                    const float4 s4 = srow4[q];
+                    const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
 #pragma unroll
-                        for (int c = 0; c < 3; ++c) {
-                            float o = 0.f;
-                            if (k < ncoef) {
-                                const float sv = srow[3 * k + c];
-                                o = bv[k] * dR[c];
-                                ax[c] += bx[k] * sv; ay[c] += by[k] * sv; az[c] += bz[k] * sv;
-                            }
-                            srow[3 * k + c] = o;
+                    for (int e = 0; e < 4; ++e) {
+                        const int k = (4 * q + e) / 3, c = (4 * q + e) % 3;
+                        if (k < ncoef) {
+                            o[e] = bv[k] * dR[c];
+                            ax[c] += bx[k] * sv[e]; ay[c] += by[k] * sv[e]; az[c] += bz[k] * sv[e];
                         }
                     }
                 }
-            } else if (M == 16) {
-                // 192 B per Gaussian in and out, through the staging block (filled above, written back below)
-                float4* srow4 = stage4 + lane * kStageStride4;
-#pragma unroll
-                for (int q = 0; q < 12; ++q) {
-                    float o[4] = {0.f, 0.f, 0.f, 0.f};
-                    if (4 * q < 3 * ncoef) {
-                        const float4 s4 = srow4[q];
-                        const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const int k = (4 * q + e) / 3, c = (4 * q + e) % 3;
-                            if (k < ncoef) {
-                                o[e] = bv[k] * dR[c];
-                                ax[c] += bx[k] * sv[e]; ay[c] += by[k] * sv[e]; az[c] += bz[k] * sv[e];
-                            }
-                        }
-                    }
-                    srow4[q] = make_float4(o[0], o[1], o[2], o[3]);
-                }
-            } else {
-                const float* sh = a.in.d_shs + i * M * 3;
-                for (int k = 0; k < M; ++k) {
-                    float o0 = 0.f, o1 = 0.f, o2 = 0.f;
-                    if (k < ncoef && k < 16) {
-                        float bvk = 0.f, bxk = 0.f, byk = 0.f, bzk = 0.f;
-#pragma unroll
-                        for (int j2 = 0; j2 < 16; ++j2)
-                            if (j2 == k) { bvk = bv[j2]; bxk = bx[j2]; byk = by[j2]; bzk = bz[j2]; }
-                        o0 = bvk * dR[0]; o1 = bvk * dR[1]; o2 = bvk * dR[2];
-                        const float s0 = sh[3 * k], s1 = sh[3 * k + 1], s2 = sh[3 * k + 2];
-                        ax[0] += bxk * s0; ax[1] += bxk * s1; ax[2] += bxk * s2;
-                        ay[0] += byk * s0; ay[1] += byk * s1; ay[2] += byk * s2;
-                        az[0] += bzk * s0; az[1] += bzk * s1; az[2] += bzk * s2;
-                    }
-                    if (write) {
-                        dsh[3 * k] = active ? o0 : 0.f; dsh[3 * k + 1] = active ? o1 : 0.f; dsh[3 * k + 2] = active ? o2 : 0.f;
-                    }
-                }
+                srow4[q] = make_float4(o[0], o[1], o[2], o[3]);
             }
             const V3 dcdx = v3(ax[0], ax[1], ax[2]), dcdy = v3(ay[0], ay[1], ay[2]), dcdz = v3(az[0], az[1], az[2]);
             // through dir = dorig / |dorig|:  d/dv = (dv |v|^2 - v (v . dv)) / |v|^3
@@ -476,21 +415,24 @@ geom_bwd_kernel(BwdArgs a) {
             for (int k = 0; k < M * 3; ++k) dsh[k] = 0.f;
         }
         // SH gradient rows back to memory, by the whole warp (has_sh and M are warp-uniform)
-        if (!kList && staged4 && !active) {
+        if (!kList && has_sh && !active) {
             // in-place walk: an unrendered lane's staged row holds whatever the garbage inputs produced: zeros go out
 #pragma unroll
             for (int q = 0; q < 12; ++q) stage4[lane * kStageStride4 + q] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
         if (kFrost) {
-            warp_scatter_rows(a.fg.d_sh_rest + i * (size_t)fr.sh_rest * 3, fr.sh_rest * 3, stage + 3, kFrostStride, rows, lane);
+            const int nf = fr.sh_rest * 3;
+            warp_scatter_rows(a.fg.d_sh_rest + i * (size_t)nf, nf, nf, stage + 3, kStageStride, rows, lane);
             if (active) {
-                a.fg.d_sh_dc[3 * i] = stage[lane * kFrostStride]; a.fg.d_sh_dc[3 * i + 1] = stage[lane * kFrostStride + 1];
-                a.fg.d_sh_dc[3 * i + 2] = stage[lane * kFrostStride + 2];
+                a.fg.d_sh_dc[3 * i] = stage[lane * kStageStride]; a.fg.d_sh_dc[3 * i + 1] = stage[lane * kStageStride + 1];
+                a.fg.d_sh_dc[3 * i + 2] = stage[lane * kStageStride + 2];
             }
             __syncwarp();
-        } else if (staged4) {
+        } else if (has_sh && M == 16) {
             if (!kList && rows == 32) warp_scatter_block4(a.g.d_dL_dsh + (size_t)jb * 48, stage4, lane);
             else warp_scatter_rows4(dsh, stage4, rows, lane);
+        } else if (has_sh) {
+            warp_scatter_rows(dsh, 3 * M, 48, stage, kStageStride, rows, lane);
         }
         if (!write) continue;
 

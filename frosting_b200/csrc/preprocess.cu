@@ -25,22 +25,6 @@ namespace fb200 {
 
 namespace {
 
-// SH basis constants, the float values nvcc materialised from DGR/cuda_rasterizer/auxiliary.h:22-39
-__device__ constexpr float kC0 = 0.28209479177387814f;
-__device__ constexpr float kC1 = 0.4886025119029199f;
-__device__ constexpr float kC2_0 = 1.0925484305920792f;
-__device__ constexpr float kC2_1 = -1.0925484305920792f;
-__device__ constexpr float kC2_2 = 0.31539156525252005f;
-__device__ constexpr float kC2_3 = -1.0925484305920792f;
-__device__ constexpr float kC2_4 = 0.5462742152960396f;
-__device__ constexpr float kC3_0 = -0.5900435899266435f;
-__device__ constexpr float kC3_1 = 2.890611442640554f;
-__device__ constexpr float kC3_2 = -0.4570457994644658f;
-__device__ constexpr float kC3_3 = 0.3731763325901154f;
-__device__ constexpr float kC3_4 = -0.4570457994644658f;
-__device__ constexpr float kC3_5 = 1.445305721320277f;
-__device__ constexpr float kC3_6 = -0.5900435899266435f;
-
 struct Cov3 {
     float c0, c1, c2, c3, c4, c5;
 };
@@ -216,12 +200,8 @@ struct CamConst {
     float campos[3];
 };
 
-#ifndef FB200_PRE_CTAS
-#define FB200_PRE_CTAS 4
-#endif
 constexpr int kPreThreads = 256;
-constexpr int kPreRounds = 1;        // one round: a longer span only serialises runs of survivors inside a few CTAs
-constexpr int kPreSpan = kPreThreads * kPreRounds;     // Gaussians per CTA
+constexpr int kPreSpan = kPreThreads;   // Gaussians per CTA: a longer span only serialises runs of survivors in a few CTAs
 
 // ---- per-tile instance counts for the 32 rectangles of a warp, warp-balanced ----
 // The reference's duplicateWithKeys walks each splat's tile rectangle in a serial per-thread double loop
@@ -400,12 +380,12 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
     a.clamped[idx] = clamp_bits;
 }
 
-// A CTA owns kPreSpan consecutive Gaussians.  Phase A: every thread culls kPreRounds of them (occlusion lookup +
-// near plane: two short load chains) and the survivors -- ~10 % of a Frosting layer under occlusion culling -- are
-// compacted into shared memory.  Phase B: the heavy part runs over the compacted list with full warps (run in place,
-// the heavy part kept only about a third of the lanes of a warp active).
+// A CTA owns kPreSpan consecutive Gaussians.  Phase A: every thread culls one of them (occlusion lookup + near plane:
+// two short load chains) and the survivors -- ~10 % of a Frosting layer under occlusion culling -- are compacted into
+// shared memory.  Phase B: the heavy part runs over the compacted list with full warps (run in place, the heavy part
+// kept only about a third of the lanes of a warp active).  4 CTAs per SM measured faster than 3 (DESIGN.md §7).
 template <bool kFrost>
-__global__ void __launch_bounds__(kPreThreads, FB200_PRE_CTAS)
+__global__ void __launch_bounds__(kPreThreads, 4)
 preprocess_fwd_kernel(FwdArgs a) {
     __shared__ CamConst cam;
     __shared__ float4 items[kPreSpan];       // {x, y, z, index bits}
@@ -427,26 +407,17 @@ preprocess_fwd_kernel(FwdArgs a) {
     // ---- phase A: cull ----
     // the occlusion inputs first: the cell -> visible-face gather is a dependent chain of its own, started before the
     // position loads so that the two chains overlap (a culled Gaussian then costs two memory round trips, not three)
-    long long cell[kPreRounds];
-    uint8_t vis_in[kPreRounds];
-#pragma unroll
-    for (int r = 0; r < kPreRounds; ++r) {
-        const int tid = base + r * kPreThreads + threadIdx.x;
-        const int idx = tid < P ? tid : P - 1;
-        const bool by_face = a.in.d_face_visible != nullptr && (long long)idx < a.in.n_cell_points;
-        cell[r] = by_face ? __ldg(a.in.d_point_cells + idx) : -1;
-        vis_in[r] = a.in.d_visibility != nullptr ? __ldg(a.in.d_visibility + idx) : (uint8_t)1;
-    }
-#pragma unroll
-    for (int r = 0; r < kPreRounds; ++r) {
-        const int tid = base + r * kPreThreads + threadIdx.x;
-        if (base + r * kPreThreads >= P) break;               // CTA-uniform
+    {
+        const int tid = base + threadIdx.x;
         const bool valid = tid < P;
         const int idx = valid ? tid : P - 1;
+        const bool by_face = a.in.d_face_visible != nullptr && (long long)idx < a.in.n_cell_points;
+        const long long cell = by_face ? __ldg(a.in.d_point_cells + idx) : -1;
+        const uint8_t vis_in = a.in.d_visibility != nullptr ? __ldg(a.in.d_visibility + idx) : (uint8_t)1;
         // occlusion culling: a per-Gaussian mask tensor, or -- without one -- render_mask = face_visible[_point_cell_indices]
         // for the mesh-bound Gaussians, True for the trailing background ones (frosting_model.py:1564-1576), looked up in place
-        const uint8_t face_in = cell[r] >= 0 ? __ldg(a.in.d_face_visible + cell[r]) : (uint8_t)1;
-        const bool shown = vis_in[r] != 0 && face_in != 0;
+        const uint8_t face_in = cell >= 0 ? __ldg(a.in.d_face_visible + cell) : (uint8_t)1;
+        const bool shown = vis_in != 0 && face_in != 0;
         float px = 0.f, py = 0.f, pz = 0.f;
         if (kFrost) {
             if (shown) { float w[6]; int vid[3]; frost_point(a.fr, (size_t)idx, w, vid, px, py, pz); }
@@ -487,7 +458,6 @@ preprocess_fwd_kernel(FwdArgs a) {
 
     // ---- phase B: project the survivors, full warps ----
     const int n = n_items;
-    static_assert(kPreRounds == 1, "phase B below handles one round (n <= kPreThreads)");
     const int jb = threadIdx.x & ~31;
     if (jb < n) {                                                       // warp-uniform
         const int j = jb + lane;
@@ -517,10 +487,8 @@ mark_visible_kernel(int P, const float* __restrict__ means, const float* __restr
 }  // namespace
 
 cudaError_t launch_preprocess_fwd(const FwdArgs& a, cudaStream_t s) {
-    const int T = a.tiles_x * a.tiles_y;
     // the per-tile counts and the counter words behind them (adjacent in the image workspace) in one memset
     const size_t span = (size_t)(reinterpret_cast<const char*>(a.counters) - reinterpret_cast<const char*>(a.tile_count)) + 64;
-    (void)T;
     cudaError_t e = cudaMemsetAsync(a.tile_count, 0, span, s);
     if (e != cudaSuccess) return e;
     if (a.prm.P > 0) {

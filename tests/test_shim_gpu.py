@@ -242,12 +242,16 @@ def test_frosting_mode_equals_the_attribute_kernel_route(cuda_device):
     """Row f1 proper: `frosting_render` (the rasterizer reads the parameters itself, nothing materialised, parameter
     gradients written by the per-Gaussian backward for rendered rows only) against `frosting_render_two_step` (attribute
     kernel -> rasterizer -> attribute backward): bit-identical image and radii, gradients equal up to the order of the
-    blend backward's float atomics; the optimizer-sink route gives the same numbers as the autograd route."""
+    blend backward's float atomics; the optimizer-sink route gives the same numbers as the autograd route.  The third
+    layer has 9 SH coefficients rendered at degree 2: a `rest` row shorter than 15 in frosting mode, and 9-coefficient
+    rows in the attribute-kernel route."""
     dev = cuda_device
-    for (W, H, P, faces, occl) in ((320, 200, 50_000, 8000, True), (200, 120, 3001, 500, False)):
+    for (W, H, P, faces, occl, M, D) in ((320, 200, 50_000, 8000, True, 16, 3), (200, 120, 3001, 500, False, 16, 3),
+                                         (320, 200, 20_000, 4000, True, 9, 2)):
         cam = scenes.make_camera(W, H, device=dev)
-        params, mesh = scenes.frosting_layer(P, cam, 11, n_faces_target=faces, device=dev, view_distance=4.5)
-        rs = scenes.settings_for(cam, 3, device=dev)
+        params, mesh = scenes.frosting_layer(P, cam, 11, n_faces_target=faces, device=dev, view_distance=4.5,
+                                             sh_coeffs=M)
+        rs = scenes.settings_for(cam, D, device=dev)
         fv = None
         if occl:
             _, fv, _ = fb.rasterize_mesh(mesh["verts"], mesh["faces"], cam.full_proj_transform, H, W, mark_last_on_bg=True)
