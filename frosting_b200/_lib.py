@@ -20,6 +20,9 @@ EXPORTED = [
     "fb200_mesh_visibility", "fb200_gaussian_mask_from_faces", "fb200_get_layout",
     "fb200_profile_enable", "fb200_profile_read", "fb200_kernel_launches",
     "fb200_frosting_attributes", "fb200_frosting_attributes_backward",
+    "fb200_frosting_forward_geometry", "fb200_frosting_forward_raster", "fb200_frosting_forward", "fb200_frosting_backward",
+    "fb200_frosting_background_attributes", "fb200_frosting_background_attributes_backward",
+    "fb200_frosting_background_struct_sizes",
     "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
@@ -80,6 +83,16 @@ class FrostingParams(C.Structure):
 class FrostingGrads(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("d_bary_logits", "d_inner_verts", "d_outer_verts", "d_opacity_logits",
                                           "d_log_scales", "d_quats", "d_sh_dc", "d_sh_rest")]
+
+
+class FrostingBackground(C.Structure):
+    _fields_ = [("n", C.c_int32)] + [(n, C.c_void_p) for n in ("d_points", "d_opacity_logits", "d_log_scales", "d_quats",
+                                                               "d_sh_dc", "d_sh_rest")]
+
+
+class FrostingBackgroundGrads(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("d_points", "d_opacity_logits", "d_log_scales", "d_quats", "d_sh_dc",
+                                          "d_sh_rest")]
 
 
 ADAM_MAX_GROUPS = 16
@@ -154,6 +167,21 @@ def lib():
     L.fb200_frosting_attributes_backward.argtypes = [C.POINTER(FrostingParams)] + [C.c_void_p] * 5 + \
         [C.POINTER(FrostingGrads), C.c_void_p]
     L.fb200_frosting_attributes_backward.restype = C.c_int
+    BG, BGG = C.POINTER(FrostingBackground), C.POINTER(FrostingBackgroundGrads)
+    L.fb200_frosting_forward_geometry.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace), BG,
+                                                  C.c_void_p, C.c_void_p]
+    L.fb200_frosting_forward_raster.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace), BG,
+                                                C.c_void_p, C.c_void_p, C.c_void_p]
+    L.fb200_frosting_forward.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace), BG,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]
+    L.fb200_frosting_backward.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace), BG,
+                                          C.c_void_p, C.c_void_p, C.POINTER(Grads), BGG, C.c_void_p]
+    L.fb200_frosting_background_attributes.argtypes = [BG, C.c_int32] + [C.c_void_p] * 6
+    L.fb200_frosting_background_attributes_backward.argtypes = [BG, C.c_int32] + [C.c_void_p] * 6 + [BGG, C.c_void_p]
+    for n in ("fb200_frosting_forward_geometry", "fb200_frosting_forward_raster", "fb200_frosting_forward",
+              "fb200_frosting_backward", "fb200_frosting_background_attributes",
+              "fb200_frosting_background_attributes_backward"):
+        getattr(L, n).restype = C.c_int
     L.fb200_loss_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.fb200_loss_partials.restype = C.c_size_t
     L.fb200_l1_dssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
@@ -188,6 +216,14 @@ def lib():
     if L.fb200_abi_struct_sizes(sizes) != 0 or [int(x) for x in sizes] != [C.sizeof(m) for m in mirrors]:
         raise RuntimeError("frosting_b200: ctypes struct mirrors out of sync with include/frosting_b200.h: "
                            f"{[int(x) for x in sizes]} vs {[C.sizeof(m) for m in mirrors]}")
+    bg_mirrors = (FrostingBackground, FrostingBackgroundGrads)
+    bg_sizes = (C.c_size_t * len(bg_mirrors))()
+    L.fb200_frosting_background_struct_sizes.argtypes = [C.POINTER(C.c_size_t)]
+    L.fb200_frosting_background_struct_sizes.restype = C.c_int
+    if L.fb200_frosting_background_struct_sizes(bg_sizes) != 0 or \
+            [int(x) for x in bg_sizes] != [C.sizeof(m) for m in bg_mirrors]:
+        raise RuntimeError("frosting_b200: background struct mirrors out of sync with include/frosting_b200.h: "
+                           f"{[int(x) for x in bg_sizes]} vs {[C.sizeof(m) for m in bg_mirrors]}")
     _lib = L
     return L
 

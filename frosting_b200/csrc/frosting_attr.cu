@@ -184,7 +184,101 @@ frosting_attr_bwd_kernel(AttrBwdArgs a) {
     reinterpret_cast<float4*>(a.g_quats)[i] = g_q;
 }
 
+// Background Gaussians (frosting_model.py:801-876): position as stored, then the same maps as a mesh row.  One thread per
+// row with plain per-row accesses: this is the cross-check of frosting mode, not a hot path.
+struct BgAttrArgs {
+    fb200_frosting_background b;
+    int R;
+    float* means3D; float* opacities; float* scales; float* rotations; float* shs;
+};
+
+struct BgAttrBwdArgs {
+    fb200_frosting_background b;
+    int R;
+    const int32_t* radii;
+    const float* g_means3D; const float* g_opacities; const float* g_scales; const float* g_rotations; const float* g_shs;
+    fb200_frosting_background_grads g;
+};
+
+__global__ void __launch_bounds__(kAttrThreads)
+frosting_bg_attr_fwd_kernel(BgAttrArgs a) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= a.b.n) return;
+    const size_t i = (size_t)idx;
+    const int R = a.R;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) a.means3D[3 * i + k] = __ldg(a.b.d_points + 3 * i + k);
+    a.opacities[i] = frost_sigmoid(__ldg(a.b.d_opacity_logits + i));
+#pragma unroll
+    for (int k = 0; k < 3; ++k) a.scales[3 * i + k] = expf(__ldg(a.b.d_log_scales + 3 * i + k));
+    float nrm;
+    reinterpret_cast<float4*>(a.rotations)[i] = frost_normalize(__ldg(reinterpret_cast<const float4*>(a.b.d_quats) + i), nrm);
+    // the output rows start at row n_mesh of a [P, M, 3] tensor: 4-byte alignment only, scalar stores
+    float* sh = a.shs + i * (size_t)(R + 1) * 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) sh[k] = __ldg(a.b.d_sh_dc + 3 * i + k);
+    const float* rest = a.b.d_sh_rest + i * (size_t)R * 3;
+    for (int k = 0; k < 3 * R; ++k) sh[3 + k] = __ldg(rest + k);
+}
+
+__global__ void __launch_bounds__(kAttrThreads)
+frosting_bg_attr_bwd_kernel(BgAttrBwdArgs a) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= a.b.n) return;
+    const size_t i = (size_t)idx;
+    const int R = a.R;
+    // with radii: an unrendered row's upstream gradients are zero by definition and may be unwritten -- not read
+    const bool live = a.radii == nullptr || a.radii[idx] > 0;
+    float gp[3] = {0.f, 0.f, 0.f}, g_ls[3] = {0.f, 0.f, 0.f}, g_op = 0.f;
+    float4 g_q = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (live) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gp[k] = a.g_means3D[3 * i + k];
+        const float sg = frost_sigmoid(__ldg(a.b.d_opacity_logits + i));
+        g_op = a.g_opacities[i] * sg * (1.0f - sg);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) g_ls[k] = a.g_scales[3 * i + k] * expf(__ldg(a.b.d_log_scales + 3 * i + k));
+        float nrm;
+        const float4 n = frost_normalize(__ldg(reinterpret_cast<const float4*>(a.b.d_quats) + i), nrm);
+        g_q = frost_normalize_backward(n, nrm, reinterpret_cast<const float4*>(a.g_rotations)[i]);
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { a.g.d_points[3 * i + k] = gp[k]; a.g.d_log_scales[3 * i + k] = g_ls[k]; }
+    a.g.d_opacity_logits[i] = g_op;
+    reinterpret_cast<float4*>(a.g.d_quats)[i] = g_q;
+    const float* gsh = a.g_shs + i * (size_t)(R + 1) * 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) a.g.d_sh_dc[3 * i + k] = live ? gsh[k] : 0.f;
+    float* grest = a.g.d_sh_rest + i * (size_t)R * 3;
+    for (int k = 0; k < 3 * R; ++k) grest[k] = live ? gsh[3 + k] : 0.f;
+}
+
 }  // namespace
+
+cudaError_t launch_frosting_bg_attr_fwd(const fb200_frosting_background& bg, int sh_rest, float* means3D,
+                                        float* opacities, float* scales, float* rotations, float* shs, cudaStream_t s) {
+    if (bg.n > 0) {
+        BgAttrArgs a; a.b = bg; a.R = sh_rest;
+        a.means3D = means3D; a.opacities = opacities; a.scales = scales; a.rotations = rotations; a.shs = shs;
+        frosting_bg_attr_fwd_kernel<<<(bg.n + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
+        count_launch();
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_frosting_bg_attr_bwd(const fb200_frosting_background& bg, int sh_rest, const int32_t* radii,
+                                        const float* g_means3D, const float* g_opacities, const float* g_scales,
+                                        const float* g_rotations, const float* g_shs,
+                                        const fb200_frosting_background_grads& g, cudaStream_t s) {
+    if (bg.n > 0) {
+        BgAttrBwdArgs a; a.b = bg; a.R = sh_rest; a.radii = radii;
+        a.g_means3D = g_means3D; a.g_opacities = g_opacities; a.g_scales = g_scales; a.g_rotations = g_rotations;
+        a.g_shs = g_shs; a.g = g;
+        frosting_bg_attr_bwd_kernel<<<(bg.n + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
+        count_launch();
+    }
+    return cudaGetLastError();
+}
 
 cudaError_t launch_frosting_attr_fwd(const fb200_frosting_params& p, float* means3D, float* opacities, float* scales,
                                      float* rotations, float* shs, cudaStream_t s) {

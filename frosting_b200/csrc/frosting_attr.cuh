@@ -88,4 +88,41 @@ __device__ __forceinline__ float4 frost_normalize_backward(float4 n, float nrm, 
     return make_float4((g.x - n.x * ng) / nrm, (g.y - n.y * ng) / nrm, (g.z - n.z * ng) / nrm, (g.w - n.w * ng) / nrm);
 }
 
+// Background Gaussians (frosting_model.py:801-876): row i of a frosting-mode frame is mesh row i of the parameter block
+// for i < P and background row i - P after them.  Both blocks go through the maps above (sigmoid, exp, normalize,
+// dc | rest); only the position differs: a background row stores it (bg_points), a mesh row builds it in its prism cell.
+// The block is chosen per row at run time: rows are contiguous, so only the warp that straddles P mixes the two.
+template <typename T>
+struct FrostRowT {
+    T* opacity_logits; T* log_scales; T* quats; T* sh_dc; T* sh_rest;   // row pointers into the owning block
+    size_t r;                                                           // row inside that block
+    bool bg;
+};
+
+__device__ __forceinline__ FrostRowT<const float> frost_row(const fb200_frosting_params& p,
+                                                            const fb200_frosting_background& b, size_t i) {
+    FrostRowT<const float> s;
+    s.bg = i >= (size_t)p.P;
+    s.r = s.bg ? i - (size_t)p.P : i;
+    s.opacity_logits = (s.bg ? b.d_opacity_logits : p.d_opacity_logits) + s.r;
+    s.log_scales = (s.bg ? b.d_log_scales : p.d_log_scales) + 3 * s.r;
+    s.quats = (s.bg ? b.d_quats : p.d_quats) + 4 * s.r;
+    s.sh_dc = (s.bg ? b.d_sh_dc : p.d_sh_dc) + 3 * s.r;
+    s.sh_rest = (s.bg ? b.d_sh_rest : p.d_sh_rest) + s.r * (size_t)p.sh_rest * 3;
+    return s;
+}
+
+__device__ __forceinline__ FrostRowT<float> frost_grad_row(const fb200_frosting_params& p, const fb200_frosting_grads& g,
+                                                           const fb200_frosting_background_grads& b, size_t i) {
+    FrostRowT<float> s;
+    s.bg = i >= (size_t)p.P;
+    s.r = s.bg ? i - (size_t)p.P : i;
+    s.opacity_logits = (s.bg ? b.d_opacity_logits : g.d_opacity_logits) + s.r;
+    s.log_scales = (s.bg ? b.d_log_scales : g.d_log_scales) + 3 * s.r;
+    s.quats = (s.bg ? b.d_quats : g.d_quats) + 4 * s.r;
+    s.sh_dc = (s.bg ? b.d_sh_dc : g.d_sh_dc) + 3 * s.r;
+    s.sh_rest = (s.bg ? b.d_sh_rest : g.d_sh_rest) + s.r * (size_t)p.sh_rest * 3;
+    return s;
+}
+
 }  // namespace fb200

@@ -209,6 +209,10 @@ geom_bwd_kernel(BwdArgs a) {
         }
         const bool write = kList ? active : in_rows;      // this lane owns an output row (zeros if it computed none)
         const size_t i = (size_t)idx;
+        // frosting mode: the row's parameters and gradient rows are in the mesh block or (idx >= fr.P) the background
+        // block; a warp may mix the two (the row movers below take one row pointer per lane).  The row pointers are
+        // re-derived where they are used (frost_row: a select between kernel parameters) rather than kept live.
+        const bool bg_row = kFrost && idx >= fr.P;
 
         float* dsh = (!kFrost && a.g.d_dL_dsh != nullptr && M > 0) ? a.g.d_dL_dsh + i * M * 3 : nullptr;
         const bool has_sh = kFrost || (a.in.d_shs != nullptr && M > 0 && dsh != nullptr);
@@ -216,18 +220,21 @@ geom_bwd_kernel(BwdArgs a) {
         auto touch = [](const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); };
         touch(a.acc + i * 12);
         if (kFrost) {
-            touch(fr.d_bary_logits + 6 * i); touch(fr.d_cells + i); touch(fr.d_log_scales + 3 * i);
-            touch(fr.d_quats + 4 * i); touch(fr.d_opacity_logits + i);
+            const FrostRowT<const float> src = frost_row(fr, a.bg, i);
+            if (bg_row) touch(a.bg.d_points + 3 * src.r);
+            else { touch(fr.d_bary_logits + 6 * i); touch(fr.d_cells + i); }
+            touch(src.log_scales); touch(src.quats); touch(src.opacity_logits);
         } else {
             touch(a.in.d_means3D + 3 * i);
             if (a.in.d_scales) { touch(a.in.d_scales + 3 * i); touch(a.in.d_rotations + 4 * i); }
         }
         if (kFrost) {
             // dc | rest rows into the staging block: [0..2] dc, [3..] rest
-            warp_gather_rows(fr.d_sh_rest + i * (size_t)fr.sh_rest * 3, fr.sh_rest * 3, stage + 3, kStageStride, rows, lane);
-            stage[lane * kStageStride + 0] = __ldg(fr.d_sh_dc + 3 * i);
-            stage[lane * kStageStride + 1] = __ldg(fr.d_sh_dc + 3 * i + 1);
-            stage[lane * kStageStride + 2] = __ldg(fr.d_sh_dc + 3 * i + 2);
+            const FrostRowT<const float> src = frost_row(fr, a.bg, i);
+            warp_gather_rows(src.sh_rest, fr.sh_rest * 3, stage + 3, kStageStride, rows, lane);
+            stage[lane * kStageStride + 0] = __ldg(src.sh_dc);
+            stage[lane * kStageStride + 1] = __ldg(src.sh_dc + 1);
+            stage[lane * kStageStride + 2] = __ldg(src.sh_dc + 2);
         } else if (has_sh && M == 16) {
             if (!kList && rows == 32) warp_gather_block4(a.in.d_shs + (size_t)jb * 48, stage4, lane);
             else warp_gather_rows4(a.in.d_shs + i * 48, stage4, rows, lane);
@@ -254,8 +261,12 @@ geom_bwd_kernel(BwdArgs a) {
         float fw[6], q_nrm = 1.f, raw_s[3] = {0.f, 0.f, 0.f};
         int fvid[3];
         float mx, my, mz;
-        if (kFrost) frost_point(fr, i, fw, fvid, mx, my, mz);
-        else { mx = a.in.d_means3D[3 * i]; my = a.in.d_means3D[3 * i + 1]; mz = a.in.d_means3D[3 * i + 2]; }
+        if (bg_row) {
+            const float* pt = a.bg.d_points + 3 * (i - (size_t)fr.P);
+            mx = __ldg(pt); my = __ldg(pt + 1); mz = __ldg(pt + 2);
+        } else if (kFrost) {
+            frost_point(fr, i, fw, fvid, mx, my, mz);
+        } else { mx = a.in.d_means3D[3 * i]; my = a.in.d_means3D[3 * i + 1]; mz = a.in.d_means3D[3 * i + 2]; }
 
         // ---- 3D covariance (recomputed from scale/rotation, or the precomputed input) ----
         float S[6];
@@ -266,9 +277,10 @@ geom_bwd_kernel(BwdArgs a) {
             const float mod = a.prm.scale_modifier;
             float4 q;
             if (kFrost) {
+                const FrostRowT<const float> src = frost_row(fr, a.bg, i);
 #pragma unroll
-                for (int k = 0; k < 3; ++k) raw_s[k] = expf(__ldg(fr.d_log_scales + 3 * i + k));
-                q = frost_normalize(__ldg(reinterpret_cast<const float4*>(fr.d_quats) + i), q_nrm);
+                for (int k = 0; k < 3; ++k) raw_s[k] = expf(__ldg(src.log_scales + k));
+                q = frost_normalize(__ldg(reinterpret_cast<const float4*>(src.quats)), q_nrm);
             } else {
                 raw_s[0] = a.in.d_scales[3 * i]; raw_s[1] = a.in.d_scales[3 * i + 1]; raw_s[2] = a.in.d_scales[3 * i + 2];
                 q = reinterpret_cast<const float4*>(a.in.d_rotations)[i];
@@ -422,10 +434,11 @@ geom_bwd_kernel(BwdArgs a) {
         }
         if (kFrost) {
             const int nf = fr.sh_rest * 3;
-            warp_scatter_rows(a.fg.d_sh_rest + i * (size_t)nf, nf, nf, stage + 3, kStageStride, rows, lane);
+            const FrostRowT<float> dst = frost_grad_row(fr, a.fg, a.bgg, i);
+            warp_scatter_rows(dst.sh_rest, nf, nf, stage + 3, kStageStride, rows, lane);
             if (active) {
-                a.fg.d_sh_dc[3 * i] = stage[lane * kStageStride]; a.fg.d_sh_dc[3 * i + 1] = stage[lane * kStageStride + 1];
-                a.fg.d_sh_dc[3 * i + 2] = stage[lane * kStageStride + 2];
+                dst.sh_dc[0] = stage[lane * kStageStride]; dst.sh_dc[1] = stage[lane * kStageStride + 1];
+                dst.sh_dc[2] = stage[lane * kStageStride + 2];
             }
             __syncwarp();
         } else if (has_sh && M == 16) {
@@ -478,17 +491,24 @@ geom_bwd_kernel(BwdArgs a) {
         }
         if (kFrost) {
             // the chain rule through the attribute maps (fb200_frosting_attributes_backward, same formulas)
-            float gb[6];
-            frost_point_backward(fr, fw, fvid, g_mean.x, g_mean.y, g_mean.z, a.fg.d_inner_verts, a.fg.d_outer_verts, gb);
-            float2* gb2 = reinterpret_cast<float2*>(a.fg.d_bary_logits + 6 * i);
-            gb2[0] = make_float2(gb[0], gb[1]); gb2[1] = make_float2(gb[2], gb[3]); gb2[2] = make_float2(gb[4], gb[5]);
-            const float sg = frost_sigmoid(__ldg(fr.d_opacity_logits + i));
-            a.fg.d_opacity_logits[i] = g_op * sg * (1.0f - sg);
-            a.fg.d_log_scales[3 * i] = g_scale.x * raw_s[0];
-            a.fg.d_log_scales[3 * i + 1] = g_scale.y * raw_s[1];
-            a.fg.d_log_scales[3 * i + 2] = g_scale.z * raw_s[2];
-            reinterpret_cast<float4*>(a.fg.d_quats)[i] =
-                frost_normalize_backward(make_float4(qr, qx, qy, qz), q_nrm, g_rot);
+            const FrostRowT<const float> src = frost_row(fr, a.bg, i);
+            const FrostRowT<float> dst = frost_grad_row(fr, a.fg, a.bgg, i);
+            if (bg_row) {
+                // a background position is a parameter itself: dL/dbg_points = dL/dmean3D
+                float* gp = a.bgg.d_points + 3 * src.r;
+                gp[0] = g_mean.x; gp[1] = g_mean.y; gp[2] = g_mean.z;
+            } else {
+                float gb[6];
+                frost_point_backward(fr, fw, fvid, g_mean.x, g_mean.y, g_mean.z, a.fg.d_inner_verts, a.fg.d_outer_verts, gb);
+                float2* gb2 = reinterpret_cast<float2*>(a.fg.d_bary_logits + 6 * i);
+                gb2[0] = make_float2(gb[0], gb[1]); gb2[1] = make_float2(gb[2], gb[3]); gb2[2] = make_float2(gb[4], gb[5]);
+            }
+            const float sg = frost_sigmoid(__ldg(src.opacity_logits));
+            dst.opacity_logits[0] = g_op * sg * (1.0f - sg);
+            dst.log_scales[0] = g_scale.x * raw_s[0];
+            dst.log_scales[1] = g_scale.y * raw_s[1];
+            dst.log_scales[2] = g_scale.z * raw_s[2];
+            *reinterpret_cast<float4*>(dst.quats) = frost_normalize_backward(make_float4(qr, qx, qy, qz), q_nrm, g_rot);
         } else {
             if (a.g.d_dL_dcolors) { a.g.d_dL_dcolors[3 * i] = g_col.x; a.g.d_dL_dcolors[3 * i + 1] = g_col.y; a.g.d_dL_dcolors[3 * i + 2] = g_col.z; }
             a.g.d_dL_dopacity[i] = g_op;

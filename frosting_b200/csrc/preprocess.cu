@@ -270,10 +270,13 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
     const float projy = fmul(hy, p_w);
 
     Cov3 S;
+    // frosting mode: the row's parameters, in the mesh block or (idx >= fr.P) the background block (frost_row: re-derived
+    // where used rather than kept live)
     if (kFrost) {
-        const float* ls = fr.d_log_scales + 3 * (size_t)idx;
+        const FrostRowT<const float> src = frost_row(fr, a.bg, (size_t)idx);
+        const float* ls = src.log_scales;
         float nrm;
-        const float4 q = frost_normalize(__ldg(reinterpret_cast<const float4*>(fr.d_quats) + idx), nrm);
+        const float4 q = frost_normalize(__ldg(reinterpret_cast<const float4*>(src.quats)), nrm);
         S = cov3d_from_scale_rot(expf(__ldg(ls)), expf(__ldg(ls + 1)), expf(__ldg(ls + 2)), a.prm.scale_modifier,
                                  q.x, q.y, q.z, q.w);
     } else if (a.in.d_cov3D_precomp != nullptr) {
@@ -324,7 +327,8 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
         const float x = __fdiv_rn(dx, len), y = __fdiv_rn(dy, len), z = __fdiv_rn(dz, len);
         float c[48];
         if (kFrost) {
-            load_sh_split(a.prm.sh_degree, fr.d_sh_dc + 3 * (size_t)idx, fr.d_sh_rest + (size_t)idx * fr.sh_rest * 3, c);
+            const FrostRowT<const float> src = frost_row(fr, a.bg, (size_t)idx);
+            load_sh_split(a.prm.sh_degree, src.sh_dc, src.sh_rest, c);
         } else {
             const float* sh = a.in.d_shs + (size_t)idx * a.prm.sh_coeffs * 3;
             if ((a.prm.sh_coeffs & 3) == 0) load_sh<true>(a.prm.sh_degree, sh, c);
@@ -342,7 +346,8 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
         const float* c = a.in.d_colors_precomp + 3 * (size_t)idx;
         cr = __ldg(c); cg = __ldg(c + 1); cb = __ldg(c + 2);
     }
-    const float opacity = kFrost ? frost_sigmoid(__ldg(fr.d_opacity_logits + idx)) : __ldg(a.in.d_opacities + idx);
+    const float opacity = kFrost ? frost_sigmoid(__ldg(frost_row(fr, a.bg, (size_t)idx).opacity_logits))
+                                 : __ldg(a.in.d_opacities + idx);
 
     // Conservative extents of {alpha >= 1/255}: |dx| > ext_x  =>  power < -t  for every dy,
     // because max_dy power = -dx^2 / (2 Sigma_xx) and Sigma_xx = cov.x (see DESIGN.md, culling).
@@ -411,16 +416,23 @@ preprocess_fwd_kernel(FwdArgs a) {
         const int tid = base + threadIdx.x;
         const bool valid = tid < P;
         const int idx = valid ? tid : P - 1;
+        // frosting mode: rows from fr.P on are background Gaussians -- no cell, no mask entry, always candidates
+        const bool bg_row = kFrost && idx >= a.fr.P;
         const bool by_face = a.in.d_face_visible != nullptr && (long long)idx < a.in.n_cell_points;
         const long long cell = by_face ? __ldg(a.in.d_point_cells + idx) : -1;
-        const uint8_t vis_in = a.in.d_visibility != nullptr ? __ldg(a.in.d_visibility + idx) : (uint8_t)1;
+        const uint8_t vis_in = a.in.d_visibility != nullptr && !bg_row ? __ldg(a.in.d_visibility + idx) : (uint8_t)1;
         // occlusion culling: a per-Gaussian mask tensor, or -- without one -- render_mask = face_visible[_point_cell_indices]
         // for the mesh-bound Gaussians, True for the trailing background ones (frosting_model.py:1564-1576), looked up in place
         const uint8_t face_in = cell >= 0 ? __ldg(a.in.d_face_visible + cell) : (uint8_t)1;
         const bool shown = vis_in != 0 && face_in != 0;
         float px = 0.f, py = 0.f, pz = 0.f;
         if (kFrost) {
-            if (shown) { float w[6]; int vid[3]; frost_point(a.fr, (size_t)idx, w, vid, px, py, pz); }
+            if (shown && bg_row) {
+                const float* pt = a.bg.d_points + 3 * (size_t)(idx - a.fr.P);
+                px = __ldg(pt); py = __ldg(pt + 1); pz = __ldg(pt + 2);
+            } else if (shown) {
+                float w[6]; int vid[3]; frost_point(a.fr, (size_t)idx, w, vid, px, py, pz);
+            }
         } else {
             px = __ldg(a.in.d_means3D + 3 * (size_t)idx + 0);
             py = __ldg(a.in.d_means3D + 3 * (size_t)idx + 1);
@@ -436,7 +448,7 @@ preprocess_fwd_kernel(FwdArgs a) {
         if (!shown) keep = false;
         if (keep) {
             // the SH row (192 B at degree 3) is consumed last, after a chain of dependent loads; start it moving now
-            const char* row = kFrost ? reinterpret_cast<const char*>(a.fr.d_sh_rest + (size_t)idx * a.fr.sh_rest * 3)
+            const char* row = kFrost ? reinterpret_cast<const char*>(frost_row(a.fr, a.bg, (size_t)idx).sh_rest)
                                      : reinterpret_cast<const char*>(a.in.d_shs + (size_t)idx * a.prm.sh_coeffs * 3);
             if (kFrost || a.in.d_shs != nullptr) {
                 asm volatile("prefetch.global.L1 [%0];" ::"l"(row));

@@ -149,10 +149,12 @@ class GradSink(dict):
 class FlatSlabs:
     """Parameter and gradient slabs + named views.  `tensors`: ordered dict name -> initial CUDA tensor."""
 
-    def __init__(self, tensors, world=1, rank=0, peer=False, group=None, rows=None):
+    def __init__(self, tensors, world=1, rank=0, peer=False, group=None, rows=None, row_names=None):
         """`rows`: when given, tensors whose first dimension equals it are row-structured (one row per Gaussian) and the
         gradient slab carries a [rows] int32 radii region behind the gradients -- peer-visible like the slab itself --
-        through which a sparse-row producer tells every rank's step which of ITS rows exist (fb200_adam_args.peer_row_radii)."""
+        through which a sparse-row producer tells every rank's step which of ITS rows exist (fb200_adam_args.peer_row_radii).
+        `row_names`: the row-structured tensors named explicitly (default: every tensor whose first dimension is `rows`;
+        a tensor that only happens to have that many rows -- Frosting's background Gaussians -- must not count)."""
         names = list(tensors)
         first = tensors[names[0]]
         if not first.is_cuda:
@@ -162,7 +164,8 @@ class FlatSlabs:
         self.starts, self.total = slab_layout([tensors[n].numel() for n in names], world)
         self.rows = int(rows) if rows else 0
         self.row_width = [tensors[n].numel() // self.rows if self.rows and tensors[n].dim() >= 1 and
-                          tensors[n].shape[0] == self.rows else 0 for n in names]
+                          tensors[n].shape[0] == self.rows and (row_names is None or n in row_names) else 0
+                          for n in names]
         self.alloc = self.total + (self.rows + 3) // 4 * 4       # elements allocated per slab: Adam's range + the radii region
         self._owned, self._opened = [], []
         self.mc_params = self.mc_grads = 0      # NVSwitch multicast mappings of the two slabs (0: none)
@@ -295,7 +298,7 @@ class FrostingAdam:
     in its backward; `opt.collect_grads()` copies autograd's `.grad` there for any other producer -- `step()` does it
     itself when nothing was written).  `state_dict()` / `load_state_dict()` speak torch.optim.Adam's format."""
 
-    def __init__(self, tensors, lrs, betas=(0.9, 0.999), eps=1e-15, group=None, average=True, rows=None):
+    def __init__(self, tensors, lrs, betas=(0.9, 0.999), eps=1e-15, group=None, average=True, rows=None, row_names=None):
         if len(tensors) > _lib.ADAM_MAX_GROUPS:
             raise ValueError(f"at most {_lib.ADAM_MAX_GROUPS} parameter groups")
         self.group = group
@@ -304,7 +307,8 @@ class FrostingAdam:
         self.rank = dist.get_rank(group) if distributed else 0
         if self.world > _lib.MAX_PEERS:
             raise ValueError(f"at most {_lib.MAX_PEERS} ranks (one NVSwitch box)")
-        self.slabs = FlatSlabs(tensors, self.world, self.rank, peer=self.world > 1, group=group, rows=rows)
+        self.slabs = FlatSlabs(tensors, self.world, self.rank, peer=self.world > 1, group=group, rows=rows,
+                               row_names=row_names)
         self.params, self.grads = self.slabs.params, self.slabs.grads
         self.param_groups = [{"name": n, "lr": float(lrs[n]), "params": [self.params[n]]} for n in self.slabs.names]
         self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
@@ -320,7 +324,9 @@ class FrostingAdam:
 
     # -- the reference's group list and schedules (frosting_optimizer.py:74-114) for the Frosting layer's tensors --
     GROUP_OF = {"bary_logits": "bary_coords", "sh_dc": "sh_coordinates_dc", "sh_rest": "sh_coordinates_rest",
-                "opacity_logits": "opacities", "log_scales": "scales", "quats": "quaternions"}
+                "opacity_logits": "opacities", "log_scales": "scales", "quats": "quaternions",
+                "bg_points": "bg_points", "bg_opacity_logits": "bg_opacities", "bg_sh_dc": "bg_sh_coordinates_dc",
+                "bg_sh_rest": "bg_sh_coordinates_rest", "bg_log_scales": "bg_scales", "bg_quats": "bg_quaternions"}
 
     @classmethod
     def for_frosting(cls, params, opt=None, spatial_lr_scale=1.0, group=None):
@@ -328,8 +334,17 @@ class FrostingAdam:
         order = ("bary_logits", "sh_dc", "sh_rest", "opacity_logits", "log_scales", "quats")
         lr = {"bary_logits": opt.position_bary_coords_lr_init, "sh_dc": opt.feature_lr, "sh_rest": opt.feature_lr / 20.0,
               "opacity_logits": opt.opacity_lr, "log_scales": opt.scaling_lr, "quats": opt.rotation_lr}
-        # one row per Gaussian in every tensor: `frosting_render` writes the rendered rows only and hands `radii` over
-        self = cls({n: params[n] for n in order}, lr, eps=1e-15, group=group, rows=params["bary_logits"].shape[0])
+        mesh_order = order
+        if "bg_points" in params:
+            # background Gaussians: the reference's six extra groups, in its order (frosting_optimizer.py:86-92)
+            order = order + ("bg_points", "bg_opacity_logits", "bg_sh_dc", "bg_sh_rest", "bg_log_scales", "bg_quats")
+            lr.update({"bg_points": opt.position_lr_init * spatial_lr_scale, "bg_opacity_logits": opt.opacity_lr,
+                       "bg_sh_dc": opt.feature_lr, "bg_sh_rest": opt.feature_lr / 20.0, "bg_log_scales": opt.scaling_lr,
+                       "bg_quats": opt.rotation_lr})
+        # one row per mesh-bound Gaussian in each of the six mesh tensors: `frosting_render` writes the rendered rows only
+        # and hands `radii` over; the background groups are dense (zero-filled rows)
+        self = cls({n: params[n] for n in order}, lr, eps=1e-15, group=group, rows=params["bary_logits"].shape[0],
+                   row_names=mesh_order)
         for g in self.param_groups:
             g["name"] = cls.GROUP_OF[g["name"]]
         self.num_iterations = opt.iterations

@@ -271,9 +271,11 @@ def _prepare(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_p
 
 
 def _prepare_frosting(frosting, rs):
-    """Frosting mode (fb200_inputs.frosting): the rasterizer reads the parameter block `fp` itself; no attribute tensors."""
-    fp, keep, device = frosting
-    P, M = int(fp.P), int(fp.sh_rest) + 1
+    """Frosting mode (fb200_inputs.frosting): the rasterizer reads the parameter block `fp` itself; no attribute tensors.
+    `frosting` = (fp, keep, device[, background block]): background Gaussians follow the fp.P mesh-bound ones."""
+    fp, keep, device = frosting[:3]
+    bgb = frosting[3] if len(frosting) > 3 else None
+    P, M = int(fp.P) + (int(bgb.n) if bgb is not None else 0), int(fp.sh_rest) + 1
     H, W = int(rs.image_height), int(rs.image_width)
     bg = _f32c(rs.bg, device, "bg")
     view = _f32c(rs.viewmatrix, device, "viewmatrix")
@@ -285,7 +287,7 @@ def _prepare_frosting(frosting, rs):
                  debug=int(bool(rs.debug)) | (2 if NO_CULL else 0), extra=None)
     inp = Inputs(d_background=_ptr(bg), d_viewmatrix=_ptr(view), d_projmatrix=_ptr(proj), d_campos=_ptr(campos),
                  n_cell_points=0, frosting=C.addressof(fp))
-    return device, P, W, H, prm, inp, (fp, keep, bg, view, proj, campos), None, None
+    return device, P, W, H, prm, inp, (fp, keep, bgb, bg, view, proj, campos), None, None
 
 
 def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -302,8 +304,14 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
     blocks at the same point, rasterizer_impl.cu:280-281), raster phase with an exactly sized buffer.
     """
     L = _lib.lib()
+    fwd_geometry, fwd_raster, fwd = L.fb200_forward_geometry, L.fb200_forward_raster, L.fb200_forward
     if frosting is not None:
         device, P, W, H, prm, inp, tensors, extra_features, extra_bg = _prepare_frosting(frosting, rs)
+        # frosting mode goes through the entry points with a background block (NULL: mesh-bound Gaussians only)
+        bgp = C.byref(frosting[3]) if len(frosting) > 3 and frosting[3] is not None else None
+        fwd_geometry = lambda prm_, inp_, ws_, *rest: L.fb200_frosting_forward_geometry(prm_, inp_, ws_, bgp, *rest)
+        fwd_raster = lambda prm_, inp_, ws_, *rest: L.fb200_frosting_forward_raster(prm_, inp_, ws_, bgp, *rest)
+        fwd = lambda prm_, inp_, ws_, *rest: L.fb200_frosting_forward(prm_, inp_, ws_, bgp, *rest)
     else:
         device, P, W, H, prm, inp, tensors, extra_features, extra_bg = _prepare(
             means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, visibility, extra_features,
@@ -341,7 +349,7 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
         pending = None
         if exact or geometry_only or EXACT_BINNING or rs.debug or hint == 0:
             # two-phase: exact count through the mailbox, then the raster phase
-            _lib.check(L.fb200_forward_geometry(C.byref(prm), C.byref(inp), C.byref(ws), rptr, sptr))
+            _lib.check(fwd_geometry(C.byref(prm), C.byref(inp), C.byref(ws), rptr, sptr))
             mailbox.copy_(status, non_blocking=True)
             stream.synchronize()
             num_rendered = int(mailbox[_lib.ST_NUM_RENDERED])
@@ -351,7 +359,7 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
                 binning = torch.empty((L.fb200_binning_bytes(capacity),), dtype=torch.uint8, device=device)
                 ws.d_binning, ws.binning_bytes, ws.binning_capacity = binning.data_ptr(), binning.numel(), capacity
                 ws.h_status = mailbox.data_ptr()     # the host HAS this frame's status words: empty sort classes are skipped
-                _lib.check(L.fb200_forward_raster(C.byref(prm), C.byref(inp), C.byref(ws),
+                _lib.check(fwd_raster(C.byref(prm), C.byref(inp), C.byref(ws),
                                                   C.c_void_p(out_color.data_ptr()), rptr, sptr))
                 ws.h_status = None
             host.hints[key] = _grow_hint(hint, num_rendered)
@@ -360,7 +368,7 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
             capacity = hint
             binning = torch.empty((L.fb200_binning_bytes(capacity),), dtype=torch.uint8, device=device)
             ws.d_binning, ws.binning_bytes, ws.binning_capacity = binning.data_ptr(), binning.numel(), capacity
-            _lib.check(L.fb200_forward(C.byref(prm), C.byref(inp), C.byref(ws), C.c_void_p(out_color.data_ptr()),
+            _lib.check(fwd(C.byref(prm), C.byref(inp), C.byref(ws), C.c_void_p(out_color.data_ptr()),
                                        rptr, sptr))
             mailbox.copy_(status, non_blocking=True)
             event.record(stream)
@@ -381,7 +389,7 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
 
 
 def _launch_backward(call: "_Call", radii, grad_out_color, grad_out_extra=None, sparse_rows=False,
-                     frosting_grads=None):
+                     frosting_grads=None, background_grads=None):
     L = _lib.lib()
     if CHECK_BEFORE_BACKWARD:
         call.check()       # a speculatively launched forward that overflowed has no state to differentiate: raise here
@@ -396,10 +404,13 @@ def _launch_backward(call: "_Call", radii, grad_out_color, grad_out_extra=None, 
         g = g.contiguous()
         if frosting_grads is not None:
             # frosting mode: the per-Gaussian backward writes the parameter gradients (rendered rows only)
+            # (mesh rows into frosting_grads, background rows -- if the forward had any -- into background_grads)
             grads = Grads(sparse_rows=1, frosting=C.addressof(frosting_grads))
-            _lib.check(L.fb200_backward(C.byref(prm), C.byref(call.inp), C.byref(call.ws),
-                                        C.c_void_p(radii.data_ptr()) if P > 0 else None,
-                                        C.c_void_p(g.data_ptr()), C.byref(grads), C.c_void_p(stream.cuda_stream)))
+            bgb = call.tensors[2]
+            _lib.check(L.fb200_frosting_backward(
+                C.byref(prm), C.byref(call.inp), C.byref(call.ws), C.byref(bgb) if bgb is not None else None,
+                C.c_void_p(radii.data_ptr()) if P > 0 else None, C.c_void_p(g.data_ptr()), C.byref(grads),
+                C.byref(background_grads) if background_grads is not None else None, C.c_void_p(stream.cuda_stream)))
             call.ws.acc_zeroed_by_forward = 0
             return None
         # one allocation carved into the gradient tensors the caller can use (each offset a multiple of 4 floats);

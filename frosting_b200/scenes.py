@@ -154,11 +154,15 @@ def uv_sphere(n_lat, n_lon, radius=3.0, centre=(0.0, 0.0, 6.0)):
 
 
 def frosting_layer(P, cam, seed, n_faces_target=1_000_000, device="cpu", sh_coeffs=16, thickness=0.02,
-                   n_min_per_cell=1, view_distance=7.5):
+                   n_min_per_cell=1, view_distance=7.5, n_background=0, behind_frac=0.25):
     """Frosting-layer scene: Gaussians bound to prism cells over a UV-sphere base mesh.
 
     Returns the *learnable parameters* (bary logits, opacity logits, log scales, raw quaternions, SH dc/rest)
     plus the mesh and `_point_cell_indices`; `frosting_attributes()` turns them into rasterizer inputs.
+    `n_background` > 0 adds Frosting's background Gaussians (the six `bg_*` keys, frosting_model.py:564-591): free
+    Gaussians outside the base mesh's bounding box, on a thick spherical shell around the scene, `behind_frac` of them
+    behind the ring cameras (radius 6 around the sphere's centre); `frosting_background_attributes()` maps them.  They
+    come from a generator of their own, so the mesh-bound tensors are the same with or without them.
     """
     g = torch.Generator().manual_seed(seed)
     n_lon = max(8, int(round(math.sqrt(n_faces_target / 2.0) * math.sqrt(2.0))))
@@ -194,9 +198,33 @@ def frosting_layer(P, cam, seed, n_faces_target=1_000_000, device="cpu", sh_coef
     params = dict(bary_logits=bary_logits, opacity_logits=opacity_logits, log_scales=log_scales, quats=quats,
                   sh_dc=sh_dc, sh_rest=sh_rest)
     mesh = dict(verts=verts, faces=faces, inner=inner, outer=outer, cells=cells)
+    if n_background > 0:
+        params.update(_background_gaussians(n_background, verts, fx, seed, sh_coeffs, behind_frac))
     params = {k: v.contiguous().to(device) for k, v in params.items()}
     mesh = {k: v.contiguous().to(device) for k, v in mesh.items()}
     return params, mesh
+
+
+def _background_gaussians(n, verts, fx, seed, sh_coeffs, behind_frac):
+    g = torch.Generator().manual_seed(seed + 0x6267)           # separate stream: the mesh-bound draws are unchanged
+    lo, hi = verts.min(0).values, verts.max(0).values
+    centre, half = (lo + hi) / 2, (hi - lo) / 2
+    n_behind = int(n * behind_frac)
+    d = torch.randn(n, 3, generator=g)
+    d[:, 1] *= 0.5                                                # flatter towards the ring's plane
+    d = d / d.norm(dim=1, keepdim=True)
+    # distance along d at which the ray leaves the bounding box: beyond it a point is background (frosting_model.py:567-574)
+    t_box = (half[None] / d.abs().clamp_min(1e-6)).min(1).values * 1.05
+    # a thick shell: in front of the ring cameras (between the box and radius 5.5, the ring being at 6) or behind them
+    u = torch.rand(n, generator=g)
+    r = t_box + u * (5.5 - t_box).clamp_min(0.0)
+    r[:n_behind] = torch.maximum(t_box[:n_behind], 7.0 + u[:n_behind] * 8.0)
+    points = centre + r[:, None] * d
+    s0 = 1.5 * r[:, None] / fx
+    log_scales = torch.log(s0) + 0.5 * torch.randn(n, 3, generator=g)
+    return dict(bg_points=points.float(), bg_opacity_logits=torch.logit(torch.rand(n, generator=g) * 0.9 + 0.05),
+                bg_log_scales=log_scales.float(), bg_quats=torch.randn(n, 4, generator=g),
+                bg_sh_dc=torch.randn(n, 1, 3, generator=g), bg_sh_rest=torch.randn(n, sh_coeffs - 1, 3, generator=g) * 0.1)
 
 
 def frosting_attributes(params, mesh):
@@ -212,4 +240,16 @@ def frosting_attributes(params, mesh):
         scales=torch.exp(params["log_scales"]),
         rotations=torch.nn.functional.normalize(params["quats"], dim=-1),
         shs=torch.cat([params["sh_dc"], params["sh_rest"]], dim=1),
+    )
+
+
+def frosting_background_attributes(params):
+    """Background parameters -> rasterizer inputs, as Frosting's bg_* properties do (frosting_model.py:801-876): points
+    as they are, sigmoid, cat(dc, rest), exp, normalize."""
+    return dict(
+        means3D=params["bg_points"],
+        opacities=torch.sigmoid(params["bg_opacity_logits"].view(-1, 1)),
+        scales=torch.exp(params["bg_log_scales"]),
+        rotations=torch.nn.functional.normalize(params["bg_quats"], dim=-1),
+        shs=torch.cat([params["bg_sh_dc"], params["bg_sh_rest"]], dim=1),
     )

@@ -140,7 +140,9 @@ typedef struct fb200_inputs {
      * no attribute tensor, in particular no [P,M,3] SH copy, is ever materialised -- and culls with
      * frosting->d_mask / frosting->d_face_visible[d_cells[i]].  prm->P == frosting->P, prm->sh_coeffs == sh_rest + 1.
      * fb200_backward then needs fb200_grads.frosting and writes the PARAMETER gradients (same chain rule as
-     * fb200_frosting_attributes_backward, inside the per-Gaussian backward kernel). */
+     * fb200_frosting_attributes_backward, inside the per-Gaussian backward kernel).  Background Gaussians (free ones after
+     * the mesh-bound rows, never culled by the mask / face lookup) come in through fb200_frosting_forward* /
+     * fb200_frosting_backward and fb200_frosting_background below; then prm->P == frosting->P + bg->n. */
     const fb200_frosting_params* frosting;
 } fb200_inputs;
 
@@ -216,7 +218,9 @@ typedef struct fb200_grads {
                                  fb200_adam_args.d_row_radii) */
     const fb200_frosting_grads* frosting; /* frosting mode (fb200_inputs.frosting): the parameter-gradient outputs; the
                                  eight pointers above may then be NULL (d_dL_dmeans2D is still written when given) and
-                                 the contract is ALWAYS sparse: only rows with radii > 0 are written */
+                                 the contract is ALWAYS sparse: only rows with radii > 0 are written -- mesh rows into
+                                 this block, background rows (fb200_frosting_backward) into fb200_frosting_background_grads
+                                 at row i - frosting->P.  The unrendered rows of both are left as they were */
 } fb200_grads;
 
 int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
@@ -257,6 +261,61 @@ int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const fl
                                        const float* d_g_opacities, const float* d_g_scales,
                                        const float* d_g_rotations, const float* d_g_shs,
                                        const fb200_frosting_grads* grads, void* stream);
+
+/* BACKGROUND GAUSSIANS of frosting mode: Frosting's free 3DGS Gaussians, concatenated after the mesh-bound ones
+ * (frosting_scene/frosting_model.py:564-591 parameters, :801-876 bg_* properties, :1415-1418 and :1487-1514 the cat).
+ * The frame is P = frosting->P + n Gaussians, mesh-bound rows first.  A background row skips the occlusion lookup (it is
+ * always a candidate, :1571-1576) and maps its parameters like a mesh row, without the prism cell:
+ *   position = d_points (used as is), opacity = sigmoid, scales = exp, rotation = normalize, SH row = dc | rest. */
+typedef struct fb200_frosting_background {
+    int32_t n;                       /* background Gaussians (0: none) */
+    const float* d_points;           /* [n,3]     _bg_points */
+    const float* d_opacity_logits;   /* [n]       _bg_opacities */
+    const float* d_log_scales;       /* [n,3]     _bg_scales */
+    const float* d_quats;            /* [n,4]     _bg_quaternions (raw), 16-byte aligned */
+    const float* d_sh_dc;            /* [n,1,3]   _bg_sh_coordinates_dc */
+    const float* d_sh_rest;          /* [n,M-1,3] _bg_sh_coordinates_rest, M - 1 = the mesh block's sh_rest */
+} fb200_frosting_background;
+
+/* Background parameter gradients: the same contract as fb200_frosting_grads (frosting mode: rows of rendered Gaussians
+ * only; the stand-alone backward: fully written).  d_quats 16-byte aligned. */
+typedef struct fb200_frosting_background_grads {
+    float* d_points; float* d_opacity_logits; float* d_log_scales; float* d_quats; float* d_sh_dc; float* d_sh_rest;
+} fb200_frosting_background_grads;
+
+/* Frosting mode with background Gaussians: fb200_forward_geometry / _raster, fb200_forward and fb200_backward with a
+ * background block (in->frosting is required; prm->P == frosting->P + bg->n).  bg == NULL or bg->n == 0: exactly the
+ * calls without it.  The backward writes the mesh rows' gradients to grads->frosting and the background rows' to
+ * bg_grads (given exactly when bg->n > 0), both for rendered rows only, row i of the frame being background row
+ * i - frosting->P. */
+int fb200_frosting_forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                                    const fb200_frosting_background* bg, int32_t* d_radii, void* stream);
+int fb200_frosting_forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                                  const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii,
+                                  void* stream);
+int fb200_frosting_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                           const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii, void* stream);
+int fb200_frosting_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                            const fb200_frosting_background* bg, const int32_t* d_radii,
+                            const float* d_dL_dout_color /* [3,H,W] */, const fb200_grads* grads,
+                            const fb200_frosting_background_grads* bg_grads, void* stream);
+
+/* The background rows' attribute maps as stand-alone kernels (the cross-check of frosting mode, like
+ * fb200_frosting_attributes).  Outputs / upstream gradients are [n, ...] rows: pass pointers offset by frosting->P rows
+ * to fill one [P, ...] tensor together with the mesh kernels.  sh_rest: M - 1.  The backward is fully written; with
+ * d_radii ([n], optional) a row with radii <= 0 gets zeros and its upstream rows are not read. */
+int fb200_frosting_background_attributes(const fb200_frosting_background* bg, int32_t sh_rest, float* d_means3D,
+                                         float* d_opacities, float* d_scales, float* d_rotations, float* d_shs,
+                                         void* stream);
+int fb200_frosting_background_attributes_backward(const fb200_frosting_background* bg, int32_t sh_rest,
+                                                  const int32_t* d_radii, const float* d_g_means3D,
+                                                  const float* d_g_opacities, const float* d_g_scales,
+                                                  const float* d_g_rotations, const float* d_g_shs,
+                                                  const fb200_frosting_background_grads* grads, void* stream);
+
+/* sizeof() of {fb200_frosting_background, fb200_frosting_background_grads} (fb200_abi_struct_sizes keeps its nine). */
+#define FB200_BACKGROUND_STRUCTS 2
+int fb200_frosting_background_struct_sizes(size_t* out /* [FB200_BACKGROUND_STRUCTS] */);
 
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).
