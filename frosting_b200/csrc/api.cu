@@ -46,47 +46,42 @@ int check_frosting(const fb200_frosting_params* fp) {
         return fail(FB200_EINVAL, "frosting_attributes: missing parameter pointer%s");
     if (fp->P > 0 && ((reinterpret_cast<uintptr_t>(fp->d_bary_logits) & 7) || (reinterpret_cast<uintptr_t>(fp->d_quats) & 15)))
         return fail(FB200_EINVAL, "frosting_attributes: bary logits must be 8-byte, quats 16-byte aligned%s");
-    return FB200_OK;
-}
-
-// background Gaussians of frosting mode (NULL: none); sh_rest is the mesh block's
-int check_background(const fb200_frosting_background* bg, int sh_rest) {
-    if (!bg) return FB200_OK;
-    if (bg->n < 0) return fail(FB200_EINVAL, "frosting background: n must be >= 0%s");
-    if (bg->n > 0 && (!bg->d_points || !bg->d_opacity_logits || !bg->d_log_scales || !bg->d_quats || !bg->d_sh_dc ||
-                      (sh_rest > 0 && !bg->d_sh_rest)))
+    // background Gaussians
+    if (fp->n_bg < 0) return fail(FB200_EINVAL, "frosting background: n_bg must be >= 0%s");
+    if (fp->n_bg > 0 && (!fp->d_bg_points || !fp->d_bg_opacity_logits || !fp->d_bg_log_scales || !fp->d_bg_quats ||
+                         !fp->d_bg_sh_dc || (fp->sh_rest > 0 && !fp->d_bg_sh_rest)))
         return fail(FB200_EINVAL, "frosting background: missing parameter pointer%s");
-    if (bg->n > 0 && (reinterpret_cast<uintptr_t>(bg->d_quats) & 15))
+    if (fp->n_bg > 0 && (reinterpret_cast<uintptr_t>(fp->d_bg_quats) & 15))
         return fail(FB200_EINVAL, "frosting background: quats must be 16-byte aligned%s");
     return FB200_OK;
 }
 
-int check_background_grads(const fb200_frosting_background_grads* g, int n, int sh_rest) {
-    if ((g != nullptr) != (n > 0))
+// the background rows of a parameter-gradient block: given exactly when there are background Gaussians
+int check_background_grads(const fb200_frosting_params* fp, const fb200_frosting_grads* g) {
+    const bool any = g->d_bg_points || g->d_bg_opacity_logits || g->d_bg_log_scales || g->d_bg_quats || g->d_bg_sh_dc ||
+                     g->d_bg_sh_rest;
+    if (any != (fp->n_bg > 0))
         return fail(FB200_EINVAL, "frosting background: give background gradients exactly when there are background "
-                                  "Gaussians (bg->n > 0)%s");
-    if (n > 0 && (!g->d_points || !g->d_opacity_logits || !g->d_log_scales || !g->d_quats || !g->d_sh_dc ||
-                  (sh_rest > 0 && !g->d_sh_rest)))
+                                  "Gaussians (n_bg > 0)%s");
+    if (fp->n_bg > 0 && (!g->d_bg_points || !g->d_bg_opacity_logits || !g->d_bg_log_scales || !g->d_bg_quats ||
+                         !g->d_bg_sh_dc || (fp->sh_rest > 0 && !g->d_bg_sh_rest)))
         return fail(FB200_EINVAL, "frosting background: gradient pointers missing%s");
-    if (n > 0 && (reinterpret_cast<uintptr_t>(g->d_quats) & 15))
+    if (fp->n_bg > 0 && (reinterpret_cast<uintptr_t>(g->d_bg_quats) & 15))
         return fail(FB200_EINVAL, "frosting background: dL/dquats must be 16-byte aligned%s");
     return FB200_OK;
 }
 
-// frosting mode (fb200_inputs.frosting): the rasterizer's own inputs are derived from the parameter block and the
-// optional background block
-int validate_frosting(const fb200_params* prm, const fb200_inputs* in, const fb200_frosting_background* bg) {
+// frosting mode (fb200_inputs.frosting): the rasterizer's own inputs are derived from the parameter block
+int validate_frosting(const fb200_params* prm, const fb200_inputs* in) {
     const fb200_frosting_params* fp = in->frosting;
     int rc = check_frosting(fp);
     if (rc != FB200_OK) return rc;
-    if ((rc = check_background(bg, fp->sh_rest)) != FB200_OK) return rc;
-    const int64_t n_bg = bg ? bg->n : 0;
     if (in->d_means3D || in->d_shs || in->d_colors_precomp || in->d_opacities || in->d_scales || in->d_rotations ||
         in->d_cov3D_precomp || in->d_visibility || in->d_point_cells || in->d_face_visible)
         return fail(FB200_EINVAL, "frosting mode: the attribute / mask pointers of fb200_inputs must be NULL%s");
-    if ((int64_t)fp->P + n_bg != prm->P || prm->sh_coeffs != fp->sh_rest + 1 || fp->sh_rest > 15)
+    if ((int64_t)fp->P + fp->n_bg != prm->P || prm->sh_coeffs != fp->sh_rest + 1 || fp->sh_rest > 15)
         return fail(FB200_EINVAL, "frosting mode: P / sh_coeffs do not match the parameter block (P = frosting->P + "
-                                  "background n, sh_rest <= 15)%s");
+                                  "frosting->n_bg, sh_rest <= 15)%s");
     if (prm->sh_degree < 0 || prm->sh_degree > 3 || (prm->sh_degree + 1) * (prm->sh_degree + 1) > prm->sh_coeffs)
         return fail(FB200_EINVAL, "sh_degree / sh_coeffs inconsistent%s");
     if ((reinterpret_cast<uintptr_t>(fp->d_quats) & 15) || (reinterpret_cast<uintptr_t>(fp->d_bary_logits) & 7))
@@ -105,8 +100,7 @@ fb200_inputs frosting_inputs(const fb200_inputs* in) {
     return r;
 }
 
-int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-             const fb200_frosting_background* bg) {
+int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws) {
     if (!prm || !in || !ws) return fail(FB200_EINVAL, "null argument struct%s");
     if (prm->P < 0 || prm->image_width <= 0 || prm->image_height <= 0)
         return fail(FB200_EINVAL, "bad extents (P >= 0, image dims > 0 required)%s");
@@ -115,7 +109,7 @@ int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_worksp
     if (prm->debug & ~3)
         return fail(FB200_EINVAL, "debug: only bits 0 (synchronise) and 1 (no sub-tile culling) are defined%s");
     if (in->frosting) {
-        int rc = validate_frosting(prm, in, bg);
+        int rc = validate_frosting(prm, in);
         if (rc != FB200_OK) return rc;
     } else if (prm->P > 0) {
         if (!in->d_means3D || !in->d_opacities) return fail(FB200_EINVAL, "means3D / opacities missing%s");
@@ -257,12 +251,6 @@ int fb200_abi_struct_sizes(size_t* out) {
     for (int i = 0; i < FB200_ABI_STRUCTS; ++i) out[i] = sizes[i];
     return FB200_OK;
 }
-int fb200_frosting_background_struct_sizes(size_t* out) {
-    if (!out) return fail(FB200_EINVAL, "frosting_background_struct_sizes: null output%s");
-    out[0] = sizeof(fb200_frosting_background);
-    out[1] = sizeof(fb200_frosting_background_grads);
-    return FB200_OK;
-}
 const char* fb200_last_error(void) { return g_err; }
 
 size_t fb200_geom_bytes(int32_t P) { return GeomLayout((size_t)(P < 0 ? 0 : P)).total; }
@@ -281,10 +269,9 @@ int fb200_get_layout(int32_t P, int32_t W, int32_t H, int64_t capacity, fb200_la
     return FB200_OK;
 }
 
-static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                     const fb200_frosting_background* bg, bool need_binning, float* d_out_color, int32_t* d_radii,
-                     FwdArgs& a) {
-    int rc = validate(prm, in, ws, bg);
+static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws, bool need_binning,
+                     float* d_out_color, int32_t* d_radii, FwdArgs& a) {
+    int rc = validate(prm, in, ws);
     if (rc != FB200_OK) return rc;
     if (prm->P > 0 && !d_radii) return fail(FB200_EINVAL, "output pointers missing%s");
     if (need_binning && !d_out_color) return fail(FB200_EINVAL, "output pointers missing%s");
@@ -298,7 +285,6 @@ static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb20
     a.prm = *prm;
     a.in = *in;
     if (in->frosting) { a.frosting = 1; a.fr = *in->frosting; a.in = frosting_inputs(in); }
-    if (bg) a.bg = *bg;
     // focal lengths exactly as rasterizer_impl.cu:222-223
     a.focal_y = prm->image_height / (2.0f * prm->tanfovy);
     a.focal_x = prm->image_width / (2.0f * prm->tanfovx);
@@ -331,12 +317,10 @@ static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb20
     return FB200_OK;
 }
 
-// The four launch sequences, each with an optional background block (frosting mode only): the plain entry points pass
-// NULL, the fb200_frosting_* ones their caller's block.
-static int forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                            const fb200_frosting_background* bg, int32_t* d_radii, void* stream) {
+int fb200_forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                           int32_t* d_radii, void* stream) {
     FwdArgs a;
-    int rc = setup_fwd(prm, in, ws, bg, false, nullptr, d_radii, a);
+    int rc = setup_fwd(prm, in, ws, false, nullptr, d_radii, a);
     if (rc != FB200_OK) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bool debug = (prm->debug & 1) != 0;
@@ -353,10 +337,10 @@ static int forward_geometry(const fb200_params* prm, const fb200_inputs* in, con
     return FB200_OK;
 }
 
-static int forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                          const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii, void* stream) {
+int fb200_forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                         float* d_out_color, int32_t* d_radii, void* stream) {
     FwdArgs a;
-    int rc = setup_fwd(prm, in, ws, bg, true, d_out_color, d_radii, a);
+    int rc = setup_fwd(prm, in, ws, true, d_out_color, d_radii, a);
     if (rc != FB200_OK) return rc;
     if ((rc = setup_extra(prm, true, false, a.ex)) != FB200_OK) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -368,20 +352,19 @@ static int forward_raster(const fb200_params* prm, const fb200_inputs* in, const
     return FB200_OK;
 }
 
-static int forward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                   const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii, void* stream) {
-    int rc = forward_geometry(prm, in, ws, bg, d_radii, stream);
+int fb200_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                  float* d_out_color, int32_t* d_radii, void* stream) {
+    int rc = fb200_forward_geometry(prm, in, ws, d_radii, stream);
     if (rc != FB200_OK) return rc;
     if (!ws) return fail(FB200_EINVAL, "null argument struct%s");
     fb200_workspace one_phase = *ws;
     one_phase.h_status = nullptr;      // nobody has synchronised: the host cannot know this frame's status words
-    return forward_raster(prm, in, &one_phase, bg, d_out_color, d_radii, stream);
+    return fb200_forward_raster(prm, in, &one_phase, d_out_color, d_radii, stream);
 }
 
-static int backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                    const fb200_frosting_background* bg, const int32_t* d_radii, const float* d_dL_dout_color,
-                    const fb200_grads* grads, const fb200_frosting_background_grads* bg_grads, void* stream) {
-    int rc = validate(prm, in, ws, bg);
+int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
+                   const int32_t* d_radii, const float* d_dL_dout_color, const fb200_grads* grads, void* stream) {
+    int rc = validate(prm, in, ws);
     if (rc != FB200_OK) return rc;
     if (!grads || !d_dL_dout_color || (prm->P > 0 && !d_radii)) return fail(FB200_EINVAL, "backward pointers missing%s");
     // outputs a caller cannot use may be NULL and are then not written: dL/dcolors on the SH path (an intermediate
@@ -395,7 +378,7 @@ static int backward(const fb200_params* prm, const fb200_inputs* in, const fb200
             return fail(FB200_EINVAL, "frosting mode: parameter-gradient pointers missing%s");
         if ((reinterpret_cast<uintptr_t>(fg->d_quats) & 15) || (reinterpret_cast<uintptr_t>(fg->d_bary_logits) & 7))
             return fail(FB200_EINVAL, "frosting mode: dL/dquats must be 16-byte aligned, dL/dbary 8-byte aligned%s");
-        if ((rc = check_background_grads(bg_grads, bg ? bg->n : 0, in->frosting->sh_rest)) != FB200_OK) return rc;
+        if ((rc = check_background_grads(in->frosting, fg)) != FB200_OK) return rc;
     } else if (fg) {
         return fail(FB200_EINVAL, "fb200_grads.frosting given without fb200_inputs.frosting%s");
     } else if (prm->P > 0 && (!grads->d_dL_dmeans2D || !grads->d_dL_dopacity || !grads->d_dL_dmeans3D ||
@@ -422,7 +405,6 @@ static int backward(const fb200_params* prm, const fb200_inputs* in, const fb200
     a.prm = *prm;
     a.in = *in;
     if (in->frosting) { a.frosting = 1; a.fr = *in->frosting; a.fg = *fg; a.in = frosting_inputs(in); }
-    if (bg && bg->n > 0) { a.bg = *bg; a.bgg = *bg_grads; }
     a.focal_y = prm->image_height / (2.0f * prm->tanfovy);
     a.focal_x = prm->image_width / (2.0f * prm->tanfovx);
     a.tiles_x = il.tiles_x; a.tiles_y = il.tiles_y;
@@ -449,57 +431,6 @@ static int backward(const fb200_params* prm, const fb200_inputs* in, const fb200
       if ((rc = stage(launch_geom_bwd(a, s), "geometry backward", debug, s)) != FB200_OK) return rc; }
     if ((rc = stage(launch_extra_grad(a, s), "extra feature gradients", debug, s)) != FB200_OK) return rc;
     return FB200_OK;
-}
-
-int fb200_forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                           int32_t* d_radii, void* stream) {
-    return forward_geometry(prm, in, ws, nullptr, d_radii, stream);
-}
-
-int fb200_forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                         float* d_out_color, int32_t* d_radii, void* stream) {
-    return forward_raster(prm, in, ws, nullptr, d_out_color, d_radii, stream);
-}
-
-int fb200_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                  float* d_out_color, int32_t* d_radii, void* stream) {
-    return forward(prm, in, ws, nullptr, d_out_color, d_radii, stream);
-}
-
-int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                   const int32_t* d_radii, const float* d_dL_dout_color, const fb200_grads* grads, void* stream) {
-    return backward(prm, in, ws, nullptr, d_radii, d_dL_dout_color, grads, nullptr, stream);
-}
-
-static int require_frosting(const fb200_inputs* in) {
-    if (!in || !in->frosting) return fail(FB200_EINVAL, "fb200_frosting_*: frosting mode (fb200_inputs.frosting) required%s");
-    return FB200_OK;
-}
-
-int fb200_frosting_forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                                    const fb200_frosting_background* bg, int32_t* d_radii, void* stream) {
-    int rc = require_frosting(in);
-    return rc != FB200_OK ? rc : forward_geometry(prm, in, ws, bg, d_radii, stream);
-}
-
-int fb200_frosting_forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                                  const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii,
-                                  void* stream) {
-    int rc = require_frosting(in);
-    return rc != FB200_OK ? rc : forward_raster(prm, in, ws, bg, d_out_color, d_radii, stream);
-}
-
-int fb200_frosting_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                           const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii, void* stream) {
-    int rc = require_frosting(in);
-    return rc != FB200_OK ? rc : forward(prm, in, ws, bg, d_out_color, d_radii, stream);
-}
-
-int fb200_frosting_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                            const fb200_frosting_background* bg, const int32_t* d_radii, const float* d_dL_dout_color,
-                            const fb200_grads* grads, const fb200_frosting_background_grads* bg_grads, void* stream) {
-    int rc = require_frosting(in);
-    return rc != FB200_OK ? rc : backward(prm, in, ws, bg, d_radii, d_dL_dout_color, grads, bg_grads, stream);
 }
 
 int fb200_mark_visible(int32_t P, const float* d_means3D, const float* d_viewmatrix, const float* d_projmatrix,
@@ -539,8 +470,11 @@ int fb200_frosting_attributes(const fb200_frosting_params* fp, float* d_means3D,
                               float* d_rotations, float* d_shs, void* stream) {
     int rc = check_frosting(fp);
     if (rc != FB200_OK) return rc;
-    if (fp->P > 0 && (!d_means3D || !d_opacities || !d_scales || !d_rotations || !d_shs))
+    const bool rows = (int64_t)fp->P + fp->n_bg > 0;
+    if (rows && (!d_means3D || !d_opacities || !d_scales || !d_rotations || !d_shs))
         return fail(FB200_EINVAL, "frosting_attributes: missing output pointer%s");
+    if (rows && (reinterpret_cast<uintptr_t>(d_rotations) & 15))
+        return fail(FB200_EINVAL, "frosting_attributes: rotations must be 16-byte aligned%s");
     return check(launch_frosting_attr_fwd(*fp, d_means3D, d_opacities, d_scales, d_rotations, d_shs,
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes");
 }
@@ -552,47 +486,18 @@ int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const fl
     int rc = check_frosting(fp);
     if (rc != FB200_OK) return rc;
     if (!grads) return fail(FB200_EINVAL, "frosting_attributes_backward: null grads%s");
-    if (fp->P > 0 && (!d_g_means3D || !d_g_opacities || !d_g_scales || !d_g_rotations || !d_g_shs ||
-                      !grads->d_bary_logits || !grads->d_opacity_logits || !grads->d_log_scales || !grads->d_quats ||
+    const bool rows = (int64_t)fp->P + fp->n_bg > 0;
+    if (rows && (!d_g_means3D || !d_g_opacities || !d_g_scales || !d_g_rotations || !d_g_shs))
+        return fail(FB200_EINVAL, "frosting_attributes_backward: missing upstream gradient pointer%s");
+    if (rows && (reinterpret_cast<uintptr_t>(d_g_rotations) & 15))
+        return fail(FB200_EINVAL, "frosting_attributes_backward: dL/drotations must be 16-byte aligned%s");
+    if (fp->P > 0 && (!grads->d_bary_logits || !grads->d_opacity_logits || !grads->d_log_scales || !grads->d_quats ||
                       !grads->d_sh_dc || (fp->sh_rest > 0 && !grads->d_sh_rest) ||
                       ((grads->d_inner_verts == nullptr) != (grads->d_outer_verts == nullptr))))
         return fail(FB200_EINVAL, "frosting_attributes_backward: missing pointer%s");
+    if ((rc = check_background_grads(fp, grads)) != FB200_OK) return rc;
     return check(launch_frosting_attr_bwd(*fp, d_g_means3D, d_g_opacities, d_g_scales, d_g_rotations, d_g_shs, *grads,
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes_backward");
-}
-
-int fb200_frosting_background_attributes(const fb200_frosting_background* bg, int32_t sh_rest, float* d_means3D,
-                                         float* d_opacities, float* d_scales, float* d_rotations, float* d_shs,
-                                         void* stream) {
-    if (!bg) return fail(FB200_EINVAL, "frosting_background_attributes: null background block%s");
-    if (sh_rest < 0) return fail(FB200_EINVAL, "frosting_background_attributes: sh_rest must be >= 0%s");
-    int rc = check_background(bg, sh_rest);
-    if (rc != FB200_OK) return rc;
-    if (bg->n > 0 && (!d_means3D || !d_opacities || !d_scales || !d_rotations || !d_shs))
-        return fail(FB200_EINVAL, "frosting_background_attributes: missing output pointer%s");
-    if (bg->n > 0 && (reinterpret_cast<uintptr_t>(d_rotations) & 15))
-        return fail(FB200_EINVAL, "frosting_background_attributes: rotations must be 16-byte aligned%s");
-    return check(launch_frosting_bg_attr_fwd(*bg, sh_rest, d_means3D, d_opacities, d_scales, d_rotations, d_shs,
-                                             static_cast<cudaStream_t>(stream)), "frosting_background_attributes");
-}
-
-int fb200_frosting_background_attributes_backward(const fb200_frosting_background* bg, int32_t sh_rest,
-                                                  const int32_t* d_radii, const float* d_g_means3D,
-                                                  const float* d_g_opacities, const float* d_g_scales,
-                                                  const float* d_g_rotations, const float* d_g_shs,
-                                                  const fb200_frosting_background_grads* grads, void* stream) {
-    if (!bg) return fail(FB200_EINVAL, "frosting_background_attributes_backward: null background block%s");
-    if (sh_rest < 0) return fail(FB200_EINVAL, "frosting_background_attributes_backward: sh_rest must be >= 0%s");
-    int rc = check_background(bg, sh_rest);
-    if (rc != FB200_OK) return rc;
-    if ((rc = check_background_grads(grads, bg->n, sh_rest)) != FB200_OK) return rc;
-    if (bg->n > 0 && (!d_g_means3D || !d_g_opacities || !d_g_scales || !d_g_rotations || !d_g_shs))
-        return fail(FB200_EINVAL, "frosting_background_attributes_backward: missing upstream gradient pointer%s");
-    if (bg->n > 0 && (reinterpret_cast<uintptr_t>(d_g_rotations) & 15))
-        return fail(FB200_EINVAL, "frosting_background_attributes_backward: dL/drotations must be 16-byte aligned%s");
-    return check(launch_frosting_bg_attr_bwd(*bg, sh_rest, d_radii, d_g_means3D, d_g_opacities, d_g_scales,
-                                             d_g_rotations, d_g_shs, *grads, static_cast<cudaStream_t>(stream)),
-                 "frosting_background_attributes_backward");
 }
 
 size_t fb200_loss_partials(int32_t C, int32_t H, int32_t W) {

@@ -185,48 +185,42 @@ frosting_attr_bwd_kernel(AttrBwdArgs a) {
 }
 
 // Background Gaussians (frosting_model.py:801-876): position as stored, then the same maps as a mesh row.  One thread per
-// row with plain per-row accesses: this is the cross-check of frosting mode, not a hot path.
-struct BgAttrArgs {
-    fb200_frosting_background b;
-    int R;
-    float* means3D; float* opacities; float* scales; float* rotations; float* shs;
-};
-
+// row with plain per-row accesses: this is the cross-check of frosting mode, not a hot path.  The output / upstream
+// gradient pointers (and `radii`) start at the first background row, row p.P of the [P + n_bg, ...] tensors.
 struct BgAttrBwdArgs {
-    fb200_frosting_background b;
-    int R;
+    fb200_frosting_params p;
     const int32_t* radii;
     const float* g_means3D; const float* g_opacities; const float* g_scales; const float* g_rotations; const float* g_shs;
-    fb200_frosting_background_grads g;
+    fb200_frosting_grads g;
 };
 
 __global__ void __launch_bounds__(kAttrThreads)
-frosting_bg_attr_fwd_kernel(BgAttrArgs a) {
+frosting_bg_attr_fwd_kernel(AttrArgs a) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= a.b.n) return;
+    if (idx >= a.p.n_bg) return;
     const size_t i = (size_t)idx;
-    const int R = a.R;
+    const int R = a.p.sh_rest;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) a.means3D[3 * i + k] = __ldg(a.b.d_points + 3 * i + k);
-    a.opacities[i] = frost_sigmoid(__ldg(a.b.d_opacity_logits + i));
+    for (int k = 0; k < 3; ++k) a.means3D[3 * i + k] = __ldg(a.p.d_bg_points + 3 * i + k);
+    a.opacities[i] = frost_sigmoid(__ldg(a.p.d_bg_opacity_logits + i));
 #pragma unroll
-    for (int k = 0; k < 3; ++k) a.scales[3 * i + k] = expf(__ldg(a.b.d_log_scales + 3 * i + k));
+    for (int k = 0; k < 3; ++k) a.scales[3 * i + k] = expf(__ldg(a.p.d_bg_log_scales + 3 * i + k));
     float nrm;
-    reinterpret_cast<float4*>(a.rotations)[i] = frost_normalize(__ldg(reinterpret_cast<const float4*>(a.b.d_quats) + i), nrm);
-    // the output rows start at row n_mesh of a [P, M, 3] tensor: 4-byte alignment only, scalar stores
+    reinterpret_cast<float4*>(a.rotations)[i] = frost_normalize(__ldg(reinterpret_cast<const float4*>(a.p.d_bg_quats) + i), nrm);
+    // the output rows start at row P of a [P + n_bg, M, 3] tensor: 4-byte alignment only, scalar stores
     float* sh = a.shs + i * (size_t)(R + 1) * 3;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) sh[k] = __ldg(a.b.d_sh_dc + 3 * i + k);
-    const float* rest = a.b.d_sh_rest + i * (size_t)R * 3;
+    for (int k = 0; k < 3; ++k) sh[k] = __ldg(a.p.d_bg_sh_dc + 3 * i + k);
+    const float* rest = a.p.d_bg_sh_rest + i * (size_t)R * 3;
     for (int k = 0; k < 3 * R; ++k) sh[3 + k] = __ldg(rest + k);
 }
 
 __global__ void __launch_bounds__(kAttrThreads)
 frosting_bg_attr_bwd_kernel(BgAttrBwdArgs a) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= a.b.n) return;
+    if (idx >= a.p.n_bg) return;
     const size_t i = (size_t)idx;
-    const int R = a.R;
+    const int R = a.p.sh_rest;
     // with radii: an unrendered row's upstream gradients are zero by definition and may be unwritten -- not read
     const bool live = a.radii == nullptr || a.radii[idx] > 0;
     float gp[3] = {0.f, 0.f, 0.f}, g_ls[3] = {0.f, 0.f, 0.f}, g_op = 0.f;
@@ -234,57 +228,38 @@ frosting_bg_attr_bwd_kernel(BgAttrBwdArgs a) {
     if (live) {
 #pragma unroll
         for (int k = 0; k < 3; ++k) gp[k] = a.g_means3D[3 * i + k];
-        const float sg = frost_sigmoid(__ldg(a.b.d_opacity_logits + i));
+        const float sg = frost_sigmoid(__ldg(a.p.d_bg_opacity_logits + i));
         g_op = a.g_opacities[i] * sg * (1.0f - sg);
 #pragma unroll
-        for (int k = 0; k < 3; ++k) g_ls[k] = a.g_scales[3 * i + k] * expf(__ldg(a.b.d_log_scales + 3 * i + k));
+        for (int k = 0; k < 3; ++k) g_ls[k] = a.g_scales[3 * i + k] * expf(__ldg(a.p.d_bg_log_scales + 3 * i + k));
         float nrm;
-        const float4 n = frost_normalize(__ldg(reinterpret_cast<const float4*>(a.b.d_quats) + i), nrm);
+        const float4 n = frost_normalize(__ldg(reinterpret_cast<const float4*>(a.p.d_bg_quats) + i), nrm);
         g_q = frost_normalize_backward(n, nrm, reinterpret_cast<const float4*>(a.g_rotations)[i]);
     }
 #pragma unroll
-    for (int k = 0; k < 3; ++k) { a.g.d_points[3 * i + k] = gp[k]; a.g.d_log_scales[3 * i + k] = g_ls[k]; }
-    a.g.d_opacity_logits[i] = g_op;
-    reinterpret_cast<float4*>(a.g.d_quats)[i] = g_q;
+    for (int k = 0; k < 3; ++k) { a.g.d_bg_points[3 * i + k] = gp[k]; a.g.d_bg_log_scales[3 * i + k] = g_ls[k]; }
+    a.g.d_bg_opacity_logits[i] = g_op;
+    reinterpret_cast<float4*>(a.g.d_bg_quats)[i] = g_q;
     const float* gsh = a.g_shs + i * (size_t)(R + 1) * 3;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) a.g.d_sh_dc[3 * i + k] = live ? gsh[k] : 0.f;
-    float* grest = a.g.d_sh_rest + i * (size_t)R * 3;
+    for (int k = 0; k < 3; ++k) a.g.d_bg_sh_dc[3 * i + k] = live ? gsh[k] : 0.f;
+    float* grest = a.g.d_bg_sh_rest + i * (size_t)R * 3;
     for (int k = 0; k < 3 * R; ++k) grest[k] = live ? gsh[3 + k] : 0.f;
 }
 
 }  // namespace
 
-cudaError_t launch_frosting_bg_attr_fwd(const fb200_frosting_background& bg, int sh_rest, float* means3D,
-                                        float* opacities, float* scales, float* rotations, float* shs, cudaStream_t s) {
-    if (bg.n > 0) {
-        BgAttrArgs a; a.b = bg; a.R = sh_rest;
-        a.means3D = means3D; a.opacities = opacities; a.scales = scales; a.rotations = rotations; a.shs = shs;
-        frosting_bg_attr_fwd_kernel<<<(bg.n + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
-        count_launch();
-    }
-    return cudaGetLastError();
-}
-
-cudaError_t launch_frosting_bg_attr_bwd(const fb200_frosting_background& bg, int sh_rest, const int32_t* radii,
-                                        const float* g_means3D, const float* g_opacities, const float* g_scales,
-                                        const float* g_rotations, const float* g_shs,
-                                        const fb200_frosting_background_grads& g, cudaStream_t s) {
-    if (bg.n > 0) {
-        BgAttrBwdArgs a; a.b = bg; a.R = sh_rest; a.radii = radii;
-        a.g_means3D = g_means3D; a.g_opacities = g_opacities; a.g_scales = g_scales; a.g_rotations = g_rotations;
-        a.g_shs = g_shs; a.g = g;
-        frosting_bg_attr_bwd_kernel<<<(bg.n + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
-        count_launch();
-    }
-    return cudaGetLastError();
-}
-
 cudaError_t launch_frosting_attr_fwd(const fb200_frosting_params& p, float* means3D, float* opacities, float* scales,
                                      float* rotations, float* shs, cudaStream_t s) {
+    AttrArgs a; a.p = p; a.means3D = means3D; a.opacities = opacities; a.scales = scales; a.rotations = rotations; a.shs = shs;
     if (p.P > 0) {
-        AttrArgs a; a.p = p; a.means3D = means3D; a.opacities = opacities; a.scales = scales; a.rotations = rotations; a.shs = shs;
         frosting_attr_fwd_kernel<<<(p.P + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
+        count_launch();
+    }
+    if (p.n_bg > 0) {
+        const size_t P = (size_t)p.P;
+        a.means3D += 3 * P; a.opacities += P; a.scales += 3 * P; a.rotations += 4 * P; a.shs += P * (p.sh_rest + 1) * 3;
+        frosting_bg_attr_fwd_kernel<<<(p.n_bg + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
         count_launch();
     }
     return cudaGetLastError();
@@ -306,6 +281,14 @@ cudaError_t launch_frosting_attr_bwd(const fb200_frosting_params& p, const float
         a.g_opacity_logits = g.d_opacity_logits; a.g_log_scales = g.d_log_scales; a.g_quats = g.d_quats;
         a.g_sh_dc = g.d_sh_dc; a.g_sh_rest = g.d_sh_rest;
         frosting_attr_bwd_kernel<<<(p.P + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(a);
+        count_launch();
+    }
+    if (p.n_bg > 0) {
+        const size_t P = (size_t)p.P;
+        BgAttrBwdArgs b; b.p = p; b.radii = p.d_radii != nullptr ? p.d_radii + P : nullptr;
+        b.g_means3D = g_means3D + 3 * P; b.g_opacities = g_opacities + P; b.g_scales = g_scales + 3 * P;
+        b.g_rotations = g_rotations + 4 * P; b.g_shs = g_shs + P * (p.sh_rest + 1) * 3; b.g = g;
+        frosting_bg_attr_bwd_kernel<<<(p.n_bg + kAttrThreads - 1) / kAttrThreads, kAttrThreads, 0, s>>>(b);
         count_launch();
     }
     return cudaGetLastError();

@@ -209,8 +209,8 @@ geom_bwd_kernel(BwdArgs a) {
         }
         const bool write = kList ? active : in_rows;      // this lane owns an output row (zeros if it computed none)
         const size_t i = (size_t)idx;
-        // frosting mode: the row's parameters and gradient rows are in the mesh block or (idx >= fr.P) the background
-        // block; a warp may mix the two (the row movers below take one row pointer per lane).  The row pointers are
+        // frosting mode: the row's parameters and gradient rows are the mesh rows or (idx >= fr.P) the d_bg_* rows of
+        // the blocks; a warp may mix the two (the row movers below take one row pointer per lane).  The row pointers are
         // re-derived where they are used (frost_row: a select between kernel parameters) rather than kept live.
         const bool bg_row = kFrost && idx >= fr.P;
 
@@ -220,8 +220,8 @@ geom_bwd_kernel(BwdArgs a) {
         auto touch = [](const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); };
         touch(a.acc + i * 12);
         if (kFrost) {
-            const FrostRowT<const float> src = frost_row(fr, a.bg, i);
-            if (bg_row) touch(a.bg.d_points + 3 * src.r);
+            const FrostRowT<const float> src = frost_row(fr, i);
+            if (bg_row) touch(fr.d_bg_points + 3 * src.r);
             else { touch(fr.d_bary_logits + 6 * i); touch(fr.d_cells + i); }
             touch(src.log_scales); touch(src.quats); touch(src.opacity_logits);
         } else {
@@ -230,7 +230,7 @@ geom_bwd_kernel(BwdArgs a) {
         }
         if (kFrost) {
             // dc | rest rows into the staging block: [0..2] dc, [3..] rest
-            const FrostRowT<const float> src = frost_row(fr, a.bg, i);
+            const FrostRowT<const float> src = frost_row(fr, i);
             warp_gather_rows(src.sh_rest, fr.sh_rest * 3, stage + 3, kStageStride, rows, lane);
             stage[lane * kStageStride + 0] = __ldg(src.sh_dc);
             stage[lane * kStageStride + 1] = __ldg(src.sh_dc + 1);
@@ -262,7 +262,7 @@ geom_bwd_kernel(BwdArgs a) {
         int fvid[3];
         float mx, my, mz;
         if (bg_row) {
-            const float* pt = a.bg.d_points + 3 * (i - (size_t)fr.P);
+            const float* pt = fr.d_bg_points + 3 * (i - (size_t)fr.P);
             mx = __ldg(pt); my = __ldg(pt + 1); mz = __ldg(pt + 2);
         } else if (kFrost) {
             frost_point(fr, i, fw, fvid, mx, my, mz);
@@ -277,7 +277,7 @@ geom_bwd_kernel(BwdArgs a) {
             const float mod = a.prm.scale_modifier;
             float4 q;
             if (kFrost) {
-                const FrostRowT<const float> src = frost_row(fr, a.bg, i);
+                const FrostRowT<const float> src = frost_row(fr, i);
 #pragma unroll
                 for (int k = 0; k < 3; ++k) raw_s[k] = expf(__ldg(src.log_scales + k));
                 q = frost_normalize(__ldg(reinterpret_cast<const float4*>(src.quats)), q_nrm);
@@ -434,7 +434,7 @@ geom_bwd_kernel(BwdArgs a) {
         }
         if (kFrost) {
             const int nf = fr.sh_rest * 3;
-            const FrostRowT<float> dst = frost_grad_row(fr, a.fg, a.bgg, i);
+            const FrostRowT<float> dst = frost_grad_row(fr, a.fg, i);
             warp_scatter_rows(dst.sh_rest, nf, nf, stage + 3, kStageStride, rows, lane);
             if (active) {
                 dst.sh_dc[0] = stage[lane * kStageStride]; dst.sh_dc[1] = stage[lane * kStageStride + 1];
@@ -491,11 +491,11 @@ geom_bwd_kernel(BwdArgs a) {
         }
         if (kFrost) {
             // the chain rule through the attribute maps (fb200_frosting_attributes_backward, same formulas)
-            const FrostRowT<const float> src = frost_row(fr, a.bg, i);
-            const FrostRowT<float> dst = frost_grad_row(fr, a.fg, a.bgg, i);
+            const FrostRowT<const float> src = frost_row(fr, i);
+            const FrostRowT<float> dst = frost_grad_row(fr, a.fg, i);
             if (bg_row) {
                 // a background position is a parameter itself: dL/dbg_points = dL/dmean3D
-                float* gp = a.bgg.d_points + 3 * src.r;
+                float* gp = a.fg.d_bg_points + 3 * src.r;
                 gp[0] = g_mean.x; gp[1] = g_mean.y; gp[2] = g_mean.z;
             } else {
                 float gb[6];

@@ -270,10 +270,10 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
     const float projy = fmul(hy, p_w);
 
     Cov3 S;
-    // frosting mode: the row's parameters, in the mesh block or (idx >= fr.P) the background block (frost_row: re-derived
-    // where used rather than kept live)
+    // frosting mode: the row's parameters, the mesh rows or (idx >= fr.P) the d_bg_* rows of the block (frost_row:
+    // re-derived where used rather than kept live)
     if (kFrost) {
-        const FrostRowT<const float> src = frost_row(fr, a.bg, (size_t)idx);
+        const FrostRowT<const float> src = frost_row(fr, (size_t)idx);
         const float* ls = src.log_scales;
         float nrm;
         const float4 q = frost_normalize(__ldg(reinterpret_cast<const float4*>(src.quats)), nrm);
@@ -327,7 +327,7 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
         const float x = __fdiv_rn(dx, len), y = __fdiv_rn(dy, len), z = __fdiv_rn(dz, len);
         float c[48];
         if (kFrost) {
-            const FrostRowT<const float> src = frost_row(fr, a.bg, (size_t)idx);
+            const FrostRowT<const float> src = frost_row(fr, (size_t)idx);
             load_sh_split(a.prm.sh_degree, src.sh_dc, src.sh_rest, c);
         } else {
             const float* sh = a.in.d_shs + (size_t)idx * a.prm.sh_coeffs * 3;
@@ -346,7 +346,7 @@ __device__ __forceinline__ void project_gaussian(const FwdArgs& a, const CamCons
         const float* c = a.in.d_colors_precomp + 3 * (size_t)idx;
         cr = __ldg(c); cg = __ldg(c + 1); cb = __ldg(c + 2);
     }
-    const float opacity = kFrost ? frost_sigmoid(__ldg(frost_row(fr, a.bg, (size_t)idx).opacity_logits))
+    const float opacity = kFrost ? frost_sigmoid(__ldg(frost_row(fr, (size_t)idx).opacity_logits))
                                  : __ldg(a.in.d_opacities + idx);
 
     // Conservative extents of {alpha >= 1/255}: |dx| > ext_x  =>  power < -t  for every dy,
@@ -428,7 +428,7 @@ preprocess_fwd_kernel(FwdArgs a) {
         float px = 0.f, py = 0.f, pz = 0.f;
         if (kFrost) {
             if (shown && bg_row) {
-                const float* pt = a.bg.d_points + 3 * (size_t)(idx - a.fr.P);
+                const float* pt = a.fr.d_bg_points + 3 * (size_t)(idx - a.fr.P);
                 px = __ldg(pt); py = __ldg(pt + 1); pz = __ldg(pt + 2);
             } else if (shown) {
                 float w[6]; int vid[3]; frost_point(a.fr, (size_t)idx, w, vid, px, py, pz);
@@ -448,7 +448,7 @@ preprocess_fwd_kernel(FwdArgs a) {
         if (!shown) keep = false;
         if (keep) {
             // the SH row (192 B at degree 3) is consumed last, after a chain of dependent loads; start it moving now
-            const char* row = kFrost ? reinterpret_cast<const char*>(frost_row(a.fr, a.bg, (size_t)idx).sh_rest)
+            const char* row = kFrost ? reinterpret_cast<const char*>(frost_row(a.fr, (size_t)idx).sh_rest)
                                      : reinterpret_cast<const char*>(a.in.d_shs + (size_t)idx * a.prm.sh_coeffs * 3);
             if (kFrost || a.in.d_shs != nullptr) {
                 asm volatile("prefetch.global.L1 [%0];" ::"l"(row));

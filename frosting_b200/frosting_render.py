@@ -29,7 +29,7 @@ import torch
 
 from . import _lib
 from . import rasterizer as R
-from ._lib import FrostingParams, FrostingGrads, FrostingBackground, FrostingBackgroundGrads
+from ._lib import FrostingParams, FrostingGrads
 
 MESH_KEYS = ("bary_logits", "opacity_logits", "log_scales", "quats", "sh_dc", "sh_rest")
 # Frosting's _bg_points, _bg_opacities, _bg_scales, _bg_quaternions, _bg_sh_coordinates_dc / _rest, in this order
@@ -50,27 +50,11 @@ def background_params(params):
     return tuple(params[k] for k in BG_KEYS)
 
 
-def _background_block(bg, dev, sh_rest):
-    """fb200_frosting_background over the six background tensors (None: no background Gaussians) and the tensors it
-    points into."""
-    if not bg or bg[0] is None:
-        return None, None
-    t = tuple(R._f32c(x, dev, "background parameter") for x in bg)
-    n = t[0].shape[0]
-    if t[0].shape != (n, 3) or t[5].shape != (n, sh_rest, 3) or any(x.shape[0] != n for x in t):
-        raise RuntimeError("background parameters must be [n,3], [n], [n,3], [n,4], [n,1,3], [n,M-1,3] with the mesh "
-                           "block's M")
-    fb = FrostingBackground(n=n, d_points=_p(t[0]), d_opacity_logits=_p(t[1]), d_log_scales=_p(t[2]), d_quats=_p(t[3]),
-                            d_sh_dc=_p(t[4]), d_sh_rest=_p(t[5]))
-    return fb, t
-
-
-def _background_grads(d):
-    return FrostingBackgroundGrads(d_points=_p(d[0]), d_opacity_logits=_p(d[1]), d_log_scales=_p(d[2]), d_quats=_p(d[3]),
-                                   d_sh_dc=_p(d[4]), d_sh_rest=_p(d[5]))
-
-
-def _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces, face_visible):
+def _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces, face_visible,
+                  bg, mask=None):
+    """fb200_frosting_params over the whole model: the mesh parameters and shell, the optional culling inputs and the
+    background parameters `bg` (BG_KEYS order; empty: none).  Returns it, the mesh-side tensors it points into
+    (parameters, inner, outer, cells, faces, face_visible, mask), the background ones (None: none) and the device."""
     if not bary_logits.is_cuda:
         raise RuntimeError("frosting_b200 runs on CUDA tensors only (no CPU fallback)")
     dev = bary_logits.device
@@ -79,13 +63,34 @@ def _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest
     cells = cells.to(device=dev, dtype=torch.int64).contiguous()
     faces = faces.to(device=dev, dtype=torch.int32).contiguous()
     fv = None if face_visible is None else face_visible.to(device=dev, dtype=torch.uint8).contiguous()
+    m = None if mask is None else mask.to(device=dev, dtype=torch.uint8).contiguous()
     P, Rn = bary_logits.shape[0], sh_rest.shape[1]
+    bg_keep = tuple(R._f32c(x, dev, "background parameter") for x in bg) if bg else None
+    b = bg_keep or (None,) * 6
+    n_bg = 0 if bg_keep is None else b[0].shape[0]
+    if bg_keep is not None and (b[0].shape != (n_bg, 3) or b[5].shape != (n_bg, Rn, 3) or
+                                any(x.shape[0] != n_bg for x in b)):
+        raise RuntimeError("background parameters must be [n,3], [n], [n,3], [n,4], [n,1,3], [n,M-1,3] with the mesh "
+                           "block's M")
     fp = FrostingParams(P=P, n_verts=inner.shape[0], n_faces=faces.shape[0], sh_rest=Rn,
                         d_bary_logits=_p(bary_logits), d_cells=_p(cells), d_faces=_p(faces),
                         d_inner_verts=_p(inner), d_outer_verts=_p(outer), d_opacity_logits=_p(opacity_logits),
                         d_log_scales=_p(log_scales), d_quats=_p(quats), d_sh_dc=_p(sh_dc), d_sh_rest=_p(sh_rest),
-                        d_mask=None, d_face_visible=_p(fv), d_radii=None)
-    return fp, (bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces, fv), dev
+                        d_mask=_p(m), d_face_visible=_p(fv), d_radii=None,
+                        n_bg=n_bg, d_bg_points=_p(b[0]), d_bg_opacity_logits=_p(b[1]), d_bg_log_scales=_p(b[2]),
+                        d_bg_quats=_p(b[3]), d_bg_sh_dc=_p(b[4]), d_bg_sh_rest=_p(b[5]))
+    keep = (bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces, fv, m)
+    return fp, keep, bg_keep, dev
+
+
+def _grads_block(d, d_in, d_out, bd):
+    """fb200_frosting_grads over the six mesh parameter gradients, the shell vertices' and the background ones (bd:
+    six tensors, or None without background Gaussians)."""
+    b = bd or (None,) * 6
+    return FrostingGrads(d_bary_logits=_p(d[0]), d_inner_verts=_p(d_in), d_outer_verts=_p(d_out),
+                         d_opacity_logits=_p(d[1]), d_log_scales=_p(d[2]), d_quats=_p(d[3]), d_sh_dc=_p(d[4]),
+                         d_sh_rest=_p(d[5]), d_bg_points=_p(b[0]), d_bg_opacity_logits=_p(b[1]),
+                         d_bg_log_scales=_p(b[2]), d_bg_quats=_p(b[3]), d_bg_sh_dc=_p(b[4]), d_bg_sh_rest=_p(b[5]))
 
 
 def _grad_targets(sink, keep, dev, radii, zero_rows, bg_keep=None):
@@ -120,8 +125,8 @@ def _grad_targets(sink, keep, dev, radii, zero_rows, bg_keep=None):
 
 
 def _returned(ctx, keep, d, d_in, d_out, bg_keep, bd):
-    """autograd's gradients for (mesh parameters, shell vertices, cells, faces, face_visible, settings, sink, background
-    parameters)."""
+    """autograd's gradients for (mesh parameters, shell vertices, the five non-differentiable inputs -- cells, faces and
+    three per-call arguments --, background parameters)."""
     tail = (None,) * 5
     if bg_keep is not None:
         tail += (None,) * 6 if ctx.sink is not None else (bd[0], bd[1].view_as(bg_keep[1])) + tuple(bd[2:])
@@ -131,15 +136,18 @@ def _returned(ctx, keep, d, d_in, d_out, bg_keep, bd):
     return (d_bary, d_op.view_as(keep[1]), d_ls, d_q, d_dc, d_rest, d_in, d_out) + tail
 
 
+def _stream(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
 class _FrostingRender(torch.autograd.Function):
     @staticmethod
     def forward(ctx, bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces,
                 face_visible, rs, sink, *bg):
-        fp, keep, dev = _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer,
-                                      cells, faces, face_visible)
-        fbg, bg_keep = _background_block(bg, dev, sh_rest.shape[1])
+        fp, keep, bg_keep, dev = _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner,
+                                               outer, cells, faces, face_visible, bg)
         color, radii, call, _ = R._launch_forward(None, None, None, None, None, None, None, rs, None,
-                                                  want_backward=True, frosting=(fp, keep, dev, fbg))
+                                                  want_backward=True, frosting=(fp, keep, dev))
         ctx.call, ctx.sink, ctx.keep, ctx.dev, ctx.bg_keep = call, sink, keep, dev, bg_keep
         ctx.vert_grad = inner.requires_grad or outer.requires_grad
         ctx.save_for_backward(radii)
@@ -151,14 +159,9 @@ class _FrostingRender(torch.autograd.Function):
         (radii,) = ctx.saved_tensors
         keep, dev, bg_keep = ctx.keep, ctx.dev, ctx.bg_keep
         d, bd = _grad_targets(ctx.sink, keep, dev, radii, zero_rows=True, bg_keep=bg_keep)
-        d_bary, d_op, d_ls, d_q, d_dc, d_rest = d
         d_in = torch.empty_like(keep[6]) if ctx.vert_grad else None
         d_out = torch.empty_like(keep[7]) if ctx.vert_grad else None
-        grads = FrostingGrads(d_bary_logits=_p(d_bary), d_inner_verts=_p(d_in), d_outer_verts=_p(d_out),
-                              d_opacity_logits=_p(d_op), d_log_scales=_p(d_ls), d_quats=_p(d_q), d_sh_dc=_p(d_dc),
-                              d_sh_rest=_p(d_rest))
-        R._launch_backward(ctx.call, radii, g_color, frosting_grads=grads,
-                           background_grads=_background_grads(bd) if bd is not None else None)
+        R._launch_backward(ctx.call, radii, g_color, frosting_grads=_grads_block(d, d_in, d_out, bd))
         return _returned(ctx, keep, d, d_in, d_out, bg_keep, bd)
 
 
@@ -168,30 +171,22 @@ class _FrostingRenderTwoStep(torch.autograd.Function):
     @staticmethod
     def forward(ctx, bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces,
                 face_visible, rs, sink, *bg):
-        fp, keep, dev = _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer,
-                                      cells, faces, face_visible)
-        fbg, bg_keep = _background_block(bg, dev, sh_rest.shape[1])
+        fp, keep, bg_keep, dev = _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner,
+                                               outer, cells, faces, face_visible, bg)
         fv = keep[10]
-        n_mesh, Rn = keep[0].shape[0], keep[5].shape[1]
-        P = n_mesh + (fbg.n if fbg is not None else 0)
+        P, Rn = fp.P + fp.n_bg, fp.sh_rest
         o = dict(dtype=torch.float32, device=dev)
         # rows of occluded Gaussians are never read by preprocess (same lookup): plain empty allocations
         means3D, opac = torch.empty((P, 3), **o), torch.empty((P, 1), **o)
         scales, rots, shs = torch.empty((P, 3), **o), torch.empty((P, 4), **o), torch.empty((P, Rn + 1, 3), **o)
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             _lib.check(_lib.lib().fb200_frosting_attributes(
-                C.byref(fp), _p(means3D), _p(opac), _p(scales), _p(rots), _p(shs), stream))
-            if fbg is not None:
-                # the background rows of the same tensors (rows n_mesh.. of one [P, ...] set: no cat)
-                _lib.check(_lib.lib().fb200_frosting_background_attributes(
-                    C.byref(fbg), Rn, *[_p(t[n_mesh:]) for t in (means3D, opac, scales, rots, shs)], stream))
+                C.byref(fp), _p(means3D), _p(opac), _p(scales), _p(rots), _p(shs), _stream(dev)))
         e = torch.Tensor([])
         color, radii, call, _ = R._launch_forward(
             means3D, shs, e, opac, scales, rots, e, rs, None, want_backward=True,
             face_visibility=(fv, keep[8]) if fv is not None else None)
-        ctx.fp, ctx.call, ctx.sink, ctx.keep, ctx.dev = fp, call, sink, keep, dev
-        ctx.fbg, ctx.bg_keep = fbg, bg_keep
+        ctx.fp, ctx.call, ctx.sink, ctx.keep, ctx.dev, ctx.bg_keep = fp, call, sink, keep, dev, bg_keep
         ctx.vert_grad = inner.requires_grad or outer.requires_grad
         ctx.save_for_backward(radii)
         ctx.mark_non_differentiable(radii)
@@ -200,29 +195,18 @@ class _FrostingRenderTwoStep(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_color, _):
         (radii,) = ctx.saved_tensors
-        keep, dev, fbg, bg_keep = ctx.keep, ctx.dev, ctx.fbg, ctx.bg_keep
+        keep, dev, bg_keep = ctx.keep, ctx.dev, ctx.bg_keep
         (dL_dmeans2D, _c, dL_dopacity, dL_dmeans3D, _cov, dL_dsh, dL_dscales, dL_drotations, _e) = R._launch_backward(
             ctx.call, radii, g_color, sparse_rows=True)
         d, bd = _grad_targets(ctx.sink, keep, dev, radii, zero_rows=False, bg_keep=bg_keep)
-        d_bary, d_op, d_ls, d_q, d_dc, d_rest = d
         d_in = torch.empty_like(keep[6]) if ctx.vert_grad else None
         d_out = torch.empty_like(keep[7]) if ctx.vert_grad else None
-        grads = FrostingGrads(d_bary_logits=_p(d_bary), d_inner_verts=_p(d_in), d_outer_verts=_p(d_out),
-                              d_opacity_logits=_p(d_op), d_log_scales=_p(d_ls), d_quats=_p(d_q), d_sh_dc=_p(d_dc),
-                              d_sh_rest=_p(d_rest))
         fp = ctx.fp
         fp.d_radii = _p(radii)
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             _lib.check(_lib.lib().fb200_frosting_attributes_backward(
                 C.byref(fp), _p(dL_dmeans3D), _p(dL_dopacity), _p(dL_dscales), _p(dL_drotations), _p(dL_dsh),
-                C.byref(grads), stream))
-            if fbg is not None:
-                n_mesh = keep[0].shape[0]
-                _lib.check(_lib.lib().fb200_frosting_background_attributes_backward(
-                    C.byref(fbg), keep[5].shape[1], _p(radii[n_mesh:]),
-                    *[_p(t[n_mesh:]) for t in (dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations, dL_dsh)],
-                    C.byref(_background_grads(bd)), stream))
+                C.byref(_grads_block(d, d_in, d_out, bd)), _stream(dev)))
         return _returned(ctx, keep, d, d_in, d_out, bg_keep, bd)
 
 

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define FB200_ABI_VERSION 5
+#define FB200_ABI_VERSION 6
 
 #define FB200_OK 0
 #define FB200_EINVAL (-1)   /* bad argument (shape / null pointer / unsupported channel count) */
@@ -80,7 +80,14 @@ typedef struct fb200_params {
 
 /* Frosting's per-frame attribute construction, fused (frosting_scene/frosting_model.py:713-799): turns the
  * model's learnable parameters into the rasterizer inputs in one kernel (and one backward kernel) instead
- * of the softmax / gather / mul / sum / sigmoid / exp / normalize / cat chain of torch ops. */
+ * of the softmax / gather / mul / sum / sigmoid / exp / normalize / cat chain of torch ops.
+ *
+ * The block describes the whole Frosting model: P mesh-bound Gaussians, then n_bg BACKGROUND Gaussians -- Frosting's
+ * free 3DGS Gaussians, concatenated after the mesh-bound ones (frosting_model.py:564-591 parameters, :801-876 bg_*
+ * properties, :1415-1418 and :1487-1514 the cat).  A frame is P + n_bg rows, mesh-bound rows first.  A background row
+ * skips the occlusion lookup (it is always a candidate, :1571-1576) and maps its parameters like a mesh row, without the
+ * prism cell: position = d_bg_points (used as is), opacity = sigmoid, scales = exp, rotation = normalize, SH row =
+ * dc | rest.  n_bg == 0: mesh-bound Gaussians only, the d_bg_* pointers are not read. */
 typedef struct fb200_frosting_params {
     int32_t P;                       /* mesh-bound Gaussians */
     int32_t n_verts, n_faces;        /* shell base mesh */
@@ -97,16 +104,27 @@ typedef struct fb200_frosting_params {
     const float* d_sh_rest;          /* [P,M-1,3] */
     const uint8_t* d_mask;           /* optional [P]: 0 = occluded, outputs for it are left untouched */
     const uint8_t* d_face_visible;   /* optional [F]: the same culling as face_visible[d_cells[i]] (no mask tensor) */
-    const int32_t* d_radii;          /* optional [P], backward only: a Gaussian with radii <= 0 was not rendered, its
-                                        upstream gradient rows are zero by definition and are NOT read (they may be
+    const int32_t* d_radii;          /* optional [P + n_bg], backward only: a Gaussian with radii <= 0 was not rendered,
+                                        its upstream gradient rows are zero by definition and are NOT read (they may be
                                         unwritten: fb200_grads.sparse_rows) */
+    int32_t n_bg;                    /* background Gaussians (0: none) */
+    const float* d_bg_points;        /* [n_bg,3]     _bg_points */
+    const float* d_bg_opacity_logits;/* [n_bg]       _bg_opacities */
+    const float* d_bg_log_scales;    /* [n_bg,3]     _bg_scales */
+    const float* d_bg_quats;         /* [n_bg,4]     _bg_quaternions (raw), 16-byte aligned */
+    const float* d_bg_sh_dc;         /* [n_bg,1,3]   _bg_sh_coordinates_dc */
+    const float* d_bg_sh_rest;       /* [n_bg,M-1,3] _bg_sh_coordinates_rest */
 } fb200_frosting_params;
 
 typedef struct fb200_frosting_grads {      /* fb200_frosting_attributes_backward: all fully written; frosting mode of
                                             * fb200_backward: rows of rendered Gaussians only.  Inner / outer vertex gradients
-                                            * are accumulated (cleared by the call first) */
+                                            * are accumulated (cleared by the call first).  The d_bg_* rows are the
+                                            * background Gaussians': given exactly when n_bg > 0, d_bg_quats 16-byte
+                                            * aligned */
     float* d_bary_logits; float* d_inner_verts; float* d_outer_verts; float* d_opacity_logits;
     float* d_log_scales; float* d_quats; float* d_sh_dc; float* d_sh_rest;
+    float* d_bg_points; float* d_bg_opacity_logits; float* d_bg_log_scales; float* d_bg_quats; float* d_bg_sh_dc;
+    float* d_bg_sh_rest;
 } fb200_frosting_grads;
 
 /* Device inputs of the forward pass.  Exactly one of (d_shs | d_colors_precomp) and exactly one of
@@ -138,11 +156,11 @@ typedef struct fb200_inputs {
      * d_point_cells and d_face_visible above must all be NULL: preprocess builds position (softmax barycentrics over the
      * prism cell), opacity (sigmoid), scales (exp), rotation (normalize) and reads the SH rows from dc | rest IN PLACE --
      * no attribute tensor, in particular no [P,M,3] SH copy, is ever materialised -- and culls with
-     * frosting->d_mask / frosting->d_face_visible[d_cells[i]].  prm->P == frosting->P, prm->sh_coeffs == sh_rest + 1.
-     * fb200_backward then needs fb200_grads.frosting and writes the PARAMETER gradients (same chain rule as
-     * fb200_frosting_attributes_backward, inside the per-Gaussian backward kernel).  Background Gaussians (free ones after
-     * the mesh-bound rows, never culled by the mask / face lookup) come in through fb200_frosting_forward* /
-     * fb200_frosting_backward and fb200_frosting_background below; then prm->P == frosting->P + bg->n. */
+     * frosting->d_mask / frosting->d_face_visible[d_cells[i]] (mesh-bound rows only: background rows are never culled).
+     * prm->P == frosting->P + frosting->n_bg, prm->sh_coeffs == sh_rest + 1.  fb200_backward then needs
+     * fb200_grads.frosting and writes the PARAMETER gradients (same chain rule as fb200_frosting_attributes_backward,
+     * inside the per-Gaussian backward kernel), row i of the frame being background row i - frosting->P when
+     * i >= frosting->P. */
     const fb200_frosting_params* frosting;
 } fb200_inputs;
 
@@ -219,8 +237,8 @@ typedef struct fb200_grads {
     const fb200_frosting_grads* frosting; /* frosting mode (fb200_inputs.frosting): the parameter-gradient outputs; the
                                  eight pointers above may then be NULL (d_dL_dmeans2D is still written when given) and
                                  the contract is ALWAYS sparse: only rows with radii > 0 are written -- mesh rows into
-                                 this block, background rows (fb200_frosting_backward) into fb200_frosting_background_grads
-                                 at row i - frosting->P.  The unrendered rows of both are left as they were */
+                                 the block's mesh gradients, background rows into its d_bg_* rows at row i - frosting->P.
+                                 The unrendered rows of both are left as they were */
 } fb200_grads;
 
 int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
@@ -253,69 +271,17 @@ int fb200_gaussian_mask_from_faces(int32_t n_points, const int64_t* d_point_cell
                                    int32_t F, const uint8_t* d_face_visible, int32_t n_background,
                                    uint8_t* d_mask, void* stream);
 
-/* Frosting's attribute construction as stand-alone kernels (structs: above, before fb200_inputs). */
-int fb200_frosting_attributes(const fb200_frosting_params* fp, float* d_means3D /*[P,3]*/, float* d_opacities /*[P,1]*/,
-                              float* d_scales /*[P,3]*/, float* d_rotations /*[P,4]*/, float* d_shs /*[P,M,3]*/,
-                              void* stream);
+/* Frosting's attribute construction as stand-alone kernels (structs: above, before fb200_inputs), the cross-check of
+ * frosting mode.  Outputs and upstream gradients have P + n_bg rows, background rows last; d_rotations and
+ * d_g_rotations 16-byte aligned.  With d_radii the backward writes zeros for a row with radii <= 0 and does not read its
+ * upstream rows. */
+int fb200_frosting_attributes(const fb200_frosting_params* fp, float* d_means3D /*[P+n_bg,3]*/,
+                              float* d_opacities /*[P+n_bg,1]*/, float* d_scales /*[P+n_bg,3]*/,
+                              float* d_rotations /*[P+n_bg,4]*/, float* d_shs /*[P+n_bg,M,3]*/, void* stream);
 int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const float* d_g_means3D,
                                        const float* d_g_opacities, const float* d_g_scales,
                                        const float* d_g_rotations, const float* d_g_shs,
                                        const fb200_frosting_grads* grads, void* stream);
-
-/* BACKGROUND GAUSSIANS of frosting mode: Frosting's free 3DGS Gaussians, concatenated after the mesh-bound ones
- * (frosting_scene/frosting_model.py:564-591 parameters, :801-876 bg_* properties, :1415-1418 and :1487-1514 the cat).
- * The frame is P = frosting->P + n Gaussians, mesh-bound rows first.  A background row skips the occlusion lookup (it is
- * always a candidate, :1571-1576) and maps its parameters like a mesh row, without the prism cell:
- *   position = d_points (used as is), opacity = sigmoid, scales = exp, rotation = normalize, SH row = dc | rest. */
-typedef struct fb200_frosting_background {
-    int32_t n;                       /* background Gaussians (0: none) */
-    const float* d_points;           /* [n,3]     _bg_points */
-    const float* d_opacity_logits;   /* [n]       _bg_opacities */
-    const float* d_log_scales;       /* [n,3]     _bg_scales */
-    const float* d_quats;            /* [n,4]     _bg_quaternions (raw), 16-byte aligned */
-    const float* d_sh_dc;            /* [n,1,3]   _bg_sh_coordinates_dc */
-    const float* d_sh_rest;          /* [n,M-1,3] _bg_sh_coordinates_rest, M - 1 = the mesh block's sh_rest */
-} fb200_frosting_background;
-
-/* Background parameter gradients: the same contract as fb200_frosting_grads (frosting mode: rows of rendered Gaussians
- * only; the stand-alone backward: fully written).  d_quats 16-byte aligned. */
-typedef struct fb200_frosting_background_grads {
-    float* d_points; float* d_opacity_logits; float* d_log_scales; float* d_quats; float* d_sh_dc; float* d_sh_rest;
-} fb200_frosting_background_grads;
-
-/* Frosting mode with background Gaussians: fb200_forward_geometry / _raster, fb200_forward and fb200_backward with a
- * background block (in->frosting is required; prm->P == frosting->P + bg->n).  bg == NULL or bg->n == 0: exactly the
- * calls without it.  The backward writes the mesh rows' gradients to grads->frosting and the background rows' to
- * bg_grads (given exactly when bg->n > 0), both for rendered rows only, row i of the frame being background row
- * i - frosting->P. */
-int fb200_frosting_forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                                    const fb200_frosting_background* bg, int32_t* d_radii, void* stream);
-int fb200_frosting_forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                                  const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii,
-                                  void* stream);
-int fb200_frosting_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                           const fb200_frosting_background* bg, float* d_out_color, int32_t* d_radii, void* stream);
-int fb200_frosting_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
-                            const fb200_frosting_background* bg, const int32_t* d_radii,
-                            const float* d_dL_dout_color /* [3,H,W] */, const fb200_grads* grads,
-                            const fb200_frosting_background_grads* bg_grads, void* stream);
-
-/* The background rows' attribute maps as stand-alone kernels (the cross-check of frosting mode, like
- * fb200_frosting_attributes).  Outputs / upstream gradients are [n, ...] rows: pass pointers offset by frosting->P rows
- * to fill one [P, ...] tensor together with the mesh kernels.  sh_rest: M - 1.  The backward is fully written; with
- * d_radii ([n], optional) a row with radii <= 0 gets zeros and its upstream rows are not read. */
-int fb200_frosting_background_attributes(const fb200_frosting_background* bg, int32_t sh_rest, float* d_means3D,
-                                         float* d_opacities, float* d_scales, float* d_rotations, float* d_shs,
-                                         void* stream);
-int fb200_frosting_background_attributes_backward(const fb200_frosting_background* bg, int32_t sh_rest,
-                                                  const int32_t* d_radii, const float* d_g_means3D,
-                                                  const float* d_g_opacities, const float* d_g_scales,
-                                                  const float* d_g_rotations, const float* d_g_shs,
-                                                  const fb200_frosting_background_grads* grads, void* stream);
-
-/* sizeof() of {fb200_frosting_background, fb200_frosting_background_grads} (fb200_abi_struct_sizes keeps its nine). */
-#define FB200_BACKGROUND_STRUCTS 2
-int fb200_frosting_background_struct_sizes(size_t* out /* [FB200_BACKGROUND_STRUCTS] */);
 
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).

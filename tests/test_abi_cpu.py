@@ -23,7 +23,7 @@ def test_every_declared_symbol_is_exported():
     for n in names:
         assert hasattr(L, n), f"{n} declared in the header but not exported"
     assert sorted(_lib.EXPORTED) == names, "frosting_b200/_lib.py:EXPORTED out of sync with the header"
-    assert L.fb200_abi_version() == _lib.ABI_VERSION == 5
+    assert L.fb200_abi_version() == _lib.ABI_VERSION == 6
 
 
 def test_workspace_size_queries_are_host_only_and_monotonic():

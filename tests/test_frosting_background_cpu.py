@@ -1,6 +1,6 @@
-"""Background Gaussians of frosting mode, host side: argument checks of the new entry points (no CUDA call is reached),
-the struct-size query, the torch restatement of Frosting's bg_* properties against the reference's own source, and the
-scene generator's compatibility with the frames it produced before."""
+"""Background Gaussians of frosting mode, host side: argument checks of the entry points (no CUDA call is reached), the
+torch restatement of Frosting's bg_* properties against the reference's own source, and the scene generator's
+compatibility with the frames it produced before."""
 import ctypes as C
 import hashlib
 import os
@@ -15,33 +15,32 @@ D = C.c_void_p(0x1000)            # 16-byte aligned dummy device pointer: never 
 ODD = C.c_void_p(0x1004)          # 4-byte aligned only
 
 
+BG = ("d_bg_points", "d_bg_opacity_logits", "d_bg_log_scales", "d_bg_quats", "d_bg_sh_dc", "d_bg_sh_rest")
+
+
 def _frame(n_mesh=10, n_bg=5):
     prm = _lib.Params(P=n_mesh + n_bg, sh_degree=3, sh_coeffs=16, image_width=64, image_height=64, tanfovx=0.5,
                       tanfovy=0.5, scale_modifier=1.0, prefiltered=0, debug=0)
     fp = _lib.FrostingParams(P=n_mesh, n_verts=4, n_faces=2, sh_rest=15, d_bary_logits=D, d_cells=D, d_faces=D,
                              d_inner_verts=D, d_outer_verts=D, d_opacity_logits=D, d_log_scales=D, d_quats=D, d_sh_dc=D,
-                             d_sh_rest=D)
+                             d_sh_rest=D, n_bg=n_bg, **{f: D for f in BG})
     inp = _lib.Inputs(d_background=D, d_viewmatrix=D, d_projmatrix=D, d_campos=D, frosting=C.addressof(fp))
-    bg = _lib.FrostingBackground(n=n_bg, d_points=D, d_opacity_logits=D, d_log_scales=D, d_quats=D, d_sh_dc=D, d_sh_rest=D)
-    bgg = _lib.FrostingBackgroundGrads(d_points=D, d_opacity_logits=D, d_log_scales=D, d_quats=D, d_sh_dc=D, d_sh_rest=D)
-    fg = _lib.FrostingGrads(d_bary_logits=D, d_opacity_logits=D, d_log_scales=D, d_quats=D, d_sh_dc=D, d_sh_rest=D)
+    fg = _lib.FrostingGrads(d_bary_logits=D, d_opacity_logits=D, d_log_scales=D, d_quats=D, d_sh_dc=D, d_sh_rest=D,
+                            **{f: D for f in BG})
     grads = _lib.Grads(sparse_rows=1, frosting=C.addressof(fg))
-    return prm, fp, inp, bg, bgg, fg, grads
+    return prm, fp, inp, fg, grads
 
 
-def _fwd(L, prm, inp, bg):
-    return L.fb200_frosting_forward(C.byref(prm), C.byref(inp), C.byref(_lib.Workspace()),
-                                    C.byref(bg) if bg is not None else None, None, None, None)
+def _fwd(L, prm, inp):
+    return L.fb200_forward(C.byref(prm), C.byref(inp), C.byref(_lib.Workspace()), None, None, None)
 
 
-def _bwd(L, prm, inp, bg, grads, bgg):
+def _bwd(L, prm, inp, grads):
     # a workspace that passes the size checks, so that the gradient checks behind them are reached; every call below
     # fails one of those, so no kernel is ever launched on these dummy pointers
     big = 1 << 40
     ws = _lib.Workspace(d_geom=D, geom_bytes=big, d_image=D, image_bytes=big, d_status=D)
-    return L.fb200_frosting_backward(C.byref(prm), C.byref(inp), C.byref(ws),
-                                     C.byref(bg) if bg is not None else None, D, D, C.byref(grads),
-                                     C.byref(bgg) if bgg is not None else None, None)
+    return L.fb200_backward(C.byref(prm), C.byref(inp), C.byref(ws), D, D, C.byref(grads), None)
 
 
 def _err(L):
@@ -51,87 +50,93 @@ def _err(L):
 def test_frosting_entry_points_reject_bad_background_arguments():
     L = _lib.lib()
     keep = _frame()
-    prm, fp, inp, bg, bgg, fg, grads = keep
-    # a valid background block gets past every frosting check (the empty workspace is the first thing missing)
-    assert _fwd(L, prm, inp, bg) == -1 and "workspace pointers missing" in _err(L)
-    for entry in (lambda b: L.fb200_frosting_forward_geometry(C.byref(prm), C.byref(inp), C.byref(_lib.Workspace()),
-                                                              C.byref(b), None, None),
-                  lambda b: L.fb200_frosting_forward_raster(C.byref(prm), C.byref(inp), C.byref(_lib.Workspace()),
-                                                            C.byref(b), None, None, None)):
-        assert entry(bg) == -1 and "workspace pointers missing" in _err(L)
-        bg.n = 4
-        assert entry(bg) == -1 and "do not match the parameter block" in _err(L)
-        bg.n = 5
-    # P != frosting->P + n
+    prm, fp, inp, fg, grads = keep
+    # valid background rows get past every frosting check (the empty workspace is the first thing missing)
+    assert _fwd(L, prm, inp) == -1 and "workspace pointers missing" in _err(L)
+    for entry in (lambda: L.fb200_forward_geometry(C.byref(prm), C.byref(inp), C.byref(_lib.Workspace()), None, None),
+                  lambda: L.fb200_forward_raster(C.byref(prm), C.byref(inp), C.byref(_lib.Workspace()), None, None,
+                                                 None)):
+        assert entry() == -1 and "workspace pointers missing" in _err(L)
+        fp.n_bg = 4
+        assert entry() == -1 and "do not match the parameter block" in _err(L)
+        fp.n_bg = 5
+    # P != frosting->P + n_bg, with and without background rows
     prm.P = 14
-    assert _fwd(L, prm, inp, bg) == -1 and "do not match the parameter block" in _err(L)
-    assert _fwd(L, prm, inp, None) == -1 and "do not match the parameter block" in _err(L)
+    assert _fwd(L, prm, inp) == -1 and "do not match the parameter block" in _err(L)
+    fp.n_bg = 0
+    assert _fwd(L, prm, inp) == -1 and "do not match the parameter block" in _err(L)
     prm.P = 10
-    assert _fwd(L, prm, inp, None) == -1 and "workspace pointers missing" in _err(L)    # NULL: the mesh-only frame
-    bg.n = 0
-    assert _fwd(L, prm, inp, bg) == -1 and "workspace pointers missing" in _err(L)      # n == 0: the same
-    bg.n = -1
-    prm.P = 9
-    assert _fwd(L, prm, inp, bg) == -1 and "n must be >= 0" in _err(L)
-    bg.n, prm.P = 5, 15
+    assert _fwd(L, prm, inp) == -1 and "workspace pointers missing" in _err(L)     # n_bg == 0: the mesh-only frame
+    fp.n_bg, prm.P = -1, 9
+    assert _fwd(L, prm, inp) == -1 and "n_bg must be >= 0" in _err(L)
+    fp.n_bg, prm.P = 5, 15
     # a missing pointer, each of the six
-    for f in ("d_points", "d_opacity_logits", "d_log_scales", "d_quats", "d_sh_dc", "d_sh_rest"):
-        setattr(bg, f, None)
-        assert _fwd(L, prm, inp, bg) == -1 and "missing parameter pointer" in _err(L), f
-        setattr(bg, f, D)
+    for f in BG:
+        setattr(fp, f, None)
+        assert _fwd(L, prm, inp) == -1 and "missing parameter pointer" in _err(L), f
+        setattr(fp, f, D)
     # misaligned quaternions, parameters and gradients
-    bg.d_quats = ODD
-    assert _fwd(L, prm, inp, bg) == -1 and "quats must be 16-byte aligned" in _err(L)
-    bg.d_quats = D
-    bgg.d_quats = ODD
-    assert _bwd(L, prm, inp, bg, grads, bgg) == -1 and "dL/dquats must be 16-byte aligned" in _err(L)
-    bgg.d_quats = D
-    for f in ("d_points", "d_opacity_logits", "d_log_scales", "d_quats", "d_sh_dc", "d_sh_rest"):
-        setattr(bgg, f, None)
-        assert _bwd(L, prm, inp, bg, grads, bgg) == -1 and "gradient pointers missing" in _err(L), f
-        setattr(bgg, f, D)
-    # gradients without parameters, parameters without gradients
-    assert _bwd(L, prm, inp, bg, grads, None) == -1 and "exactly when there are background" in _err(L)
-    prm.P = 10
-    assert _bwd(L, prm, inp, None, grads, bgg) == -1 and "exactly when there are background" in _err(L)
-    # the new entry points are frosting mode only
-    inp.frosting = None
-    assert _fwd(L, prm, inp, bg) == -1 and "frosting mode (fb200_inputs.frosting) required" in _err(L)
+    fp.d_bg_quats = ODD
+    assert _fwd(L, prm, inp) == -1 and "quats must be 16-byte aligned" in _err(L)
+    fp.d_bg_quats = D
+    fg.d_bg_quats = ODD
+    assert _bwd(L, prm, inp, grads) == -1 and "dL/dquats must be 16-byte aligned" in _err(L)
+    fg.d_bg_quats = D
+    for f in BG:
+        setattr(fg, f, None)
+        assert _bwd(L, prm, inp, grads) == -1 and "gradient pointers missing" in _err(L), f
+        setattr(fg, f, D)
+    # parameters without gradients, gradients without parameters
+    for f in BG:
+        setattr(fg, f, None)
+    assert _bwd(L, prm, inp, grads) == -1 and "exactly when there are background" in _err(L)
+    for f in BG:
+        setattr(fg, f, D)
+    fp.n_bg, prm.P = 0, 10
+    assert _bwd(L, prm, inp, grads) == -1 and "exactly when there are background" in _err(L)
+    del keep
 
 
 def test_background_attribute_entry_points_reject_bad_arguments():
     L = _lib.lib()
-    _, _, _, bg, bgg, _, _ = keep = _frame()
+    _, fp, _, fg, _ = keep = _frame()
     out = [D] * 5
-    assert L.fb200_frosting_background_attributes(None, 15, *out, None) == -1 and "null background" in _err(L)
-    assert L.fb200_frosting_background_attributes(C.byref(bg), -1, *out, None) == -1 and "sh_rest" in _err(L)
-    assert L.fb200_frosting_background_attributes(C.byref(bg), 15, D, D, D, ODD, D, None) == -1 and \
-        "rotations must be 16-byte aligned" in _err(L)
-    assert L.fb200_frosting_background_attributes(C.byref(bg), 15, D, None, D, D, D, None) == -1 and \
-        "missing output pointer" in _err(L)
-    bg.d_quats = ODD
-    assert L.fb200_frosting_background_attributes(C.byref(bg), 15, *out, None) == -1 and "quats must be" in _err(L)
-    bg.d_quats = D
     up = [D] * 5
-    assert L.fb200_frosting_background_attributes_backward(C.byref(bg), 15, None, *up, None, None) == -1 and \
+    # the kernels store rotation rows as float4: a misaligned base is rejected, with and without background rows
+    for n_bg in (5, 0):
+        fp.n_bg = n_bg
+        assert L.fb200_frosting_attributes(C.byref(fp), D, D, D, ODD, D, None) == -1 and \
+            "rotations must be 16-byte aligned" in _err(L)
+        fg_bg = [getattr(fg, f) for f in BG]
+        for f in BG:
+            setattr(fg, f, D if n_bg else None)
+        assert L.fb200_frosting_attributes_backward(C.byref(fp), D, D, D, ODD, D, C.byref(fg), None) == -1 and \
+            "dL/drotations must be 16-byte aligned" in _err(L)
+        for f, v in zip(BG, fg_bg):
+            setattr(fg, f, v)
+    fp.n_bg = 5
+    assert L.fb200_frosting_attributes(C.byref(fp), D, None, D, D, D, None) == -1 and \
+        "missing output pointer" in _err(L)
+    fp.d_bg_quats = ODD
+    assert L.fb200_frosting_attributes(C.byref(fp), *out, None) == -1 and "quats must be" in _err(L)
+    fp.d_bg_quats = D
+    for f in BG:
+        setattr(fg, f, None)
+    assert L.fb200_frosting_attributes_backward(C.byref(fp), *up, C.byref(fg), None) == -1 and \
         "exactly when there are background" in _err(L)
-    bgg.d_sh_dc = None
-    assert L.fb200_frosting_background_attributes_backward(C.byref(bg), 15, None, *up, C.byref(bgg), None) == -1 and \
+    for f in BG:
+        setattr(fg, f, D)
+    fg.d_bg_sh_dc = None
+    assert L.fb200_frosting_attributes_backward(C.byref(fp), *up, C.byref(fg), None) == -1 and \
         "gradient pointers missing" in _err(L)
-    bgg.d_sh_dc = D
-    assert L.fb200_frosting_background_attributes_backward(C.byref(bg), 15, None, D, D, D, ODD, D, C.byref(bgg),
-                                                           None) == -1 and "dL/drotations" in _err(L)
-    assert L.fb200_frosting_background_attributes_backward(C.byref(bg), 15, None, D, None, D, D, D, C.byref(bgg),
-                                                           None) == -1 and "upstream gradient" in _err(L)
+    fg.d_bg_sh_dc = D
+    fg.d_bg_quats = ODD
+    assert L.fb200_frosting_attributes_backward(C.byref(fp), *up, C.byref(fg), None) == -1 and \
+        "dL/dquats must be 16-byte aligned" in _err(L)
+    fg.d_bg_quats = D
+    assert L.fb200_frosting_attributes_backward(C.byref(fp), D, None, D, D, D, C.byref(fg), None) == -1 and \
+        "upstream gradient" in _err(L)
     del keep
-
-
-def test_background_struct_sizes_match_the_mirrors():
-    L = _lib.lib()
-    out = (C.c_size_t * 2)()
-    assert L.fb200_frosting_background_struct_sizes(out) == 0
-    assert list(out) == [C.sizeof(_lib.FrostingBackground), C.sizeof(_lib.FrostingBackgroundGrads)] == [56, 48]
-    assert L.fb200_frosting_background_struct_sizes(None) == -1
 
 
 def test_torch_background_properties_match_the_reference_goldens():

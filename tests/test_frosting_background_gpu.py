@@ -134,8 +134,8 @@ def test_background_behind_the_camera_changes_nothing(cuda_device):
 
 
 def test_background_attribute_kernels_against_the_reference_property_goldens(cuda_device):
-    """fb200_frosting_background_attributes / _backward against vectors produced by executing the reference's bg_*
-    property source (tests/golden/make_frosting_attr_golden.py): values 1e-6, gradients 2e-5 of scale."""
+    """The background rows of fb200_frosting_attributes / _backward against vectors produced by executing the reference's
+    bg_* property source (tests/golden/make_frosting_attr_golden.py): values 1e-6, gradients 2e-5 of scale."""
     dev = cuda_device
     z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "frosting_bg_attrs.npz"))
     n_mesh = 37           # a few mesh rows in front: the background rows are written behind them, in place
