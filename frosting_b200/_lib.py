@@ -20,6 +20,7 @@ EXPORTED = [
     "fb200_mesh_visibility", "fb200_gaussian_mask_from_faces", "fb200_get_layout",
     "fb200_profile_enable", "fb200_profile_read", "fb200_kernel_launches",
     "fb200_frosting_attributes", "fb200_frosting_attributes_backward",
+    "fb200_frosting_edit_shell", "fb200_frosting_edit_attributes", "fb200_frosting_edit_struct_size",
     "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
@@ -85,6 +86,20 @@ class FrostingGrads(C.Structure):
                                           "d_log_scales", "d_quats", "d_sh_dc", "d_sh_rest", "d_bg_points",
                                           "d_bg_opacity_logits", "d_bg_log_scales", "d_bg_quats", "d_bg_sh_dc",
                                           "d_bg_sh_rest")]
+
+
+RESCALE_MEDIAN, RESCALE_TRIANGLE = 0, 1
+EDIT_SELECT_WORDS = 2051
+
+
+class FrostingEdit(C.Structure):
+    _fields_ = [("n_verts", C.c_int32), ("n_faces", C.c_int32), ("rescaling", C.c_int32), ("n_edited", C.c_int32),
+                ("deformation_threshold", C.c_float)] + \
+               [(n, C.c_void_p) for n in ("d_base_verts", "d_faces", "d_inner_dist", "d_outer_dist", "d_edition_mask",
+                                          "d_verts_edition_mask", "d_vf_offsets", "d_vf_faces", "d_ref_quats",
+                                          "d_ref_dists", "d_ref_median", "d_dists", "d_face_normals", "d_rel_quats",
+                                          "d_face_factor", "d_face_keep", "d_factor", "d_select", "d_inner_verts",
+                                          "d_outer_verts")]
 
 
 ADAM_MAX_GROUPS = 16
@@ -159,6 +174,12 @@ def lib():
     L.fb200_frosting_attributes_backward.argtypes = [C.POINTER(FrostingParams)] + [C.c_void_p] * 5 + \
         [C.POINTER(FrostingGrads), C.c_void_p]
     L.fb200_frosting_attributes_backward.restype = C.c_int
+    L.fb200_frosting_edit_shell.argtypes = [C.POINTER(FrostingEdit), C.c_void_p]
+    L.fb200_frosting_edit_shell.restype = C.c_int
+    L.fb200_frosting_edit_attributes.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams), C.c_int32] + \
+        [C.c_void_p] * 8
+    L.fb200_frosting_edit_attributes.restype = C.c_int
+    L.fb200_frosting_edit_struct_size.restype = C.c_size_t
     L.fb200_loss_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.fb200_loss_partials.restype = C.c_size_t
     L.fb200_l1_dssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
@@ -193,6 +214,8 @@ def lib():
     if L.fb200_abi_struct_sizes(sizes) != 0 or [int(x) for x in sizes] != [C.sizeof(m) for m in mirrors]:
         raise RuntimeError("frosting_b200: ctypes struct mirrors out of sync with include/frosting_b200.h: "
                            f"{[int(x) for x in sizes]} vs {[C.sizeof(m) for m in mirrors]}")
+    if L.fb200_frosting_edit_struct_size() != C.sizeof(FrostingEdit):
+        raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_edit out of sync with include/frosting_b200.h")
     _lib = L
     return L
 

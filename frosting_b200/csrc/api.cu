@@ -500,6 +500,58 @@ int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const fl
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes_backward");
 }
 
+static int check_edit(const fb200_frosting_edit* e) {
+    if (!e) return fail(FB200_EINVAL, "frosting_edit: null edit struct%s");
+    if (e->n_verts < 0 || e->n_faces < 0 || e->n_edited < 0 || e->n_edited > e->n_faces)
+        return fail(FB200_EINVAL, "frosting_edit: bad extents%s");
+    if (e->rescaling != FB200_RESCALE_MEDIAN && e->rescaling != FB200_RESCALE_TRIANGLE)
+        return fail(FB200_EINVAL, "frosting_edit: unknown thickness rescaling method (median = 0, triangle = 1)%s");
+    if (e->n_faces > 0 && (!e->d_base_verts || !e->d_faces || !e->d_edition_mask || !e->d_dists || !e->d_face_normals ||
+                           !e->d_rel_quats || !e->d_face_factor || !e->d_face_keep))
+        return fail(FB200_EINVAL, "frosting_edit: missing face table pointer%s");
+    if (e->n_verts > 0 && (!e->d_inner_dist || !e->d_outer_dist || !e->d_verts_edition_mask || !e->d_vf_offsets ||
+                           !e->d_vf_faces || !e->d_inner_verts || !e->d_outer_verts))
+        return fail(FB200_EINVAL, "frosting_edit: missing vertex table pointer%s");
+    if (!e->d_factor || !e->d_select) return fail(FB200_EINVAL, "frosting_edit: missing factor / select scratch%s");
+    const bool capture = !e->d_ref_quats && !e->d_ref_dists && !e->d_ref_median;
+    if (!capture && (!e->d_ref_quats || !e->d_ref_dists || (e->rescaling == FB200_RESCALE_MEDIAN && !e->d_ref_median)))
+        return fail(FB200_EINVAL, "frosting_edit: give every reference table (or none to capture one)%s");
+    if ((reinterpret_cast<uintptr_t>(e->d_rel_quats) & 15) || (reinterpret_cast<uintptr_t>(e->d_ref_quats) & 15))
+        return fail(FB200_EINVAL, "frosting_edit: quaternion tables must be 16-byte aligned%s");
+    return FB200_OK;
+}
+
+size_t fb200_frosting_edit_struct_size(void) { return sizeof(fb200_frosting_edit); }
+
+int fb200_frosting_edit_shell(const fb200_frosting_edit* e, void* stream) {
+    int rc = check_edit(e);
+    if (rc != FB200_OK) return rc;
+    if (e->rescaling == FB200_RESCALE_MEDIAN && e->n_edited == 0)
+        return fail(FB200_EINVAL, "frosting_edit: median rescaling needs at least one edited face%s");
+    return check(launch_frosting_edit_shell(*e, static_cast<cudaStream_t>(stream)), "frosting_edit_shell");
+}
+
+int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
+                                   const float* d_campos, const float* d_orig_quats, float* d_means3D,
+                                   float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
+                                   void* stream) {
+    int rc = check_edit(e);
+    if (rc != FB200_OK) return rc;
+    if ((rc = check_frosting(fp)) != FB200_OK) return rc;
+    if (fp->n_faces != e->n_faces || fp->n_verts != e->n_verts)
+        return fail(FB200_EINVAL, "frosting_edit: the parameter block's mesh does not match the edit's%s");
+    if (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > fp->sh_rest + 1)
+        return fail(FB200_EINVAL, "frosting_edit: sh_degree needs (sh_degree + 1)^2 <= sh_rest + 1 <= 16%s");
+    const bool rows = (int64_t)fp->P + fp->n_bg > 0;
+    if (rows && (!d_campos || !d_means3D || !d_opacities || !d_scales || !d_rotations || !d_colors))
+        return fail(FB200_EINVAL, "frosting_edit: missing output pointer%s");
+    if ((reinterpret_cast<uintptr_t>(d_rotations) & 15) || (reinterpret_cast<uintptr_t>(d_orig_quats) & 15))
+        return fail(FB200_EINVAL, "frosting_edit: rotations / orig quats must be 16-byte aligned%s");
+    return check(launch_frosting_edit_attr(*e, *fp, sh_degree, d_campos, d_orig_quats, d_means3D, d_opacities, d_scales,
+                                           d_rotations, d_colors, static_cast<cudaStream_t>(stream)),
+                 "frosting_edit_attributes");
+}
+
 size_t fb200_loss_partials(int32_t C, int32_t H, int32_t W) {
     return (C > 0 && H > 0 && W > 0) ? l1_dssim_num_partials(C, H, W) : 0;
 }

@@ -253,3 +253,179 @@ def frosting_background_attributes(params):
         rotations=torch.nn.functional.normalize(params["bg_quats"], dim=-1),
         shs=torch.cat([params["bg_sh_dc"], params["bg_sh_rest"]], dim=1),
     )
+
+
+# ---- edited / animated scenes (SURVEY.md row a21): the simple adaptation of make_editable, restated ----
+# pytorch3d pieces (Meshes normals, matrix_to_quaternion, quaternion_multiply / invert / to_matrix), restated from their
+# documented definitions: pytorch3d is not a dependency.  The golden generator (tests/golden/make_frosting_edit_golden.py)
+# runs the reference's own source on top of these same restatements, so they are restated, not pinned.
+
+def p3d_faces_normals(verts, faces):
+    """Meshes.faces_normals_packed: cross(v1 - v0, v2 - v0) / max(|.|, 1e-6)."""
+    fv = verts[faces.long()]
+    n = torch.linalg.cross(fv[:, 1] - fv[:, 0], fv[:, 2] - fv[:, 0], dim=-1)
+    return n / n.norm(dim=-1, keepdim=True).clamp_min(1e-6)
+
+
+def p3d_verts_normals(verts, faces):
+    """Meshes.verts_normals_packed: the area-weighted face normals cross(v2 - v1, v0 - v1) summed per vertex, normalised
+    with eps 1e-6."""
+    fl = faces.long()
+    fv = verts[fl]
+    fn = torch.linalg.cross(fv[:, 2] - fv[:, 1], fv[:, 0] - fv[:, 1], dim=-1)
+    n = torch.zeros_like(verts)
+    for k in range(3):
+        n = n.index_add(0, fl[:, k], fn)
+    return torch.nn.functional.normalize(n, eps=1e-6, dim=1)
+
+
+def standardize_quaternion(q):
+    return torch.where(q[..., :1] < 0, -q, q)
+
+
+def quaternion_multiply(a, b):
+    """Hamilton product of (w, x, y, z) quaternions, real part made non-negative."""
+    aw, ax, ay, az = a.unbind(-1)
+    bw, bx, by, bz = b.unbind(-1)
+    return standardize_quaternion(torch.stack([
+        aw * bw - ax * bx - ay * by - az * bz,
+        aw * bx + ax * bw + ay * bz - az * by,
+        aw * by - ax * bz + ay * bw + az * bx,
+        aw * bz + ax * by - ay * bx + az * bw], -1))
+
+
+def quaternion_invert(q):
+    return q * q.new_tensor([1.0, -1.0, -1.0, -1.0])
+
+
+def quaternion_to_matrix(q):
+    r, i, j, k = q.unbind(-1)
+    two_s = 2.0 / (q * q).sum(-1)
+    m = torch.stack([1 - two_s * (j * j + k * k), two_s * (i * j - k * r), two_s * (i * k + j * r),
+                     two_s * (i * j + k * r), 1 - two_s * (i * i + k * k), two_s * (j * k - i * r),
+                     two_s * (i * k - j * r), two_s * (j * k + i * r), 1 - two_s * (i * i + j * j)], -1)
+    return m.reshape(q.shape[:-1] + (3, 3))
+
+
+def matrix_to_quaternion(m):
+    """The candidate quaternion of the largest |q_c| (first on ties), over 2 max(|q_c|, 0.1); standardised."""
+    m00, m01, m02, m10, m11, m12, m20, m21, m22 = m.reshape(m.shape[:-2] + (9,)).unbind(-1)
+    arg = torch.stack([1 + m00 + m11 + m22, 1 + m00 - m11 - m22, 1 - m00 + m11 - m22, 1 - m00 - m11 + m22], -1)
+    qa = torch.where(arg > 0, arg.clamp_min(0).sqrt(), torch.zeros_like(arg))
+    cand = torch.stack([
+        torch.stack([qa[..., 0] ** 2, m21 - m12, m02 - m20, m10 - m01], -1),
+        torch.stack([m21 - m12, qa[..., 1] ** 2, m10 + m01, m02 + m20], -1),
+        torch.stack([m02 - m20, m10 + m01, qa[..., 2] ** 2, m12 + m21], -1),
+        torch.stack([m10 - m01, m20 + m02, m21 + m12, qa[..., 3] ** 2], -1)], -2)
+    cand = cand / (2.0 * qa[..., None].clamp_min(0.1))
+    pick = qa.argmax(-1)
+    return standardize_quaternion(torch.gather(cand, -2, pick[..., None, None].expand(pick.shape + (1, 4)))[..., 0, :])
+
+
+_SH_C0, _SH_C1 = 0.28209479177387814, 0.4886025119029199
+_SH_C2 = (1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396)
+_SH_C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658,
+          1.445305721320277, -0.5900435899266435)
+
+
+def sh_colors(shs, dirs, deg):
+    """RGB of SH rows `shs` [N,M,3] (M >= (deg+1)^2) at unit directions [N,3]: the 3DGS basis, + 0.5, clamp_min 0."""
+    x, y, z = (d[:, None] for d in dirs.unbind(-1))
+    c = shs
+    r = _SH_C0 * c[:, 0]
+    if deg > 0:
+        r = r - _SH_C1 * y * c[:, 1] + _SH_C1 * z * c[:, 2] - _SH_C1 * x * c[:, 3]
+    if deg > 1:
+        xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
+        r = (r + _SH_C2[0] * xy * c[:, 4] + _SH_C2[1] * yz * c[:, 5] + _SH_C2[2] * (2 * zz - xx - yy) * c[:, 6]
+             + _SH_C2[3] * xz * c[:, 7] + _SH_C2[4] * (xx - yy) * c[:, 8])
+    if deg > 2:
+        r = (r + _SH_C3[0] * y * (3 * xx - yy) * c[:, 9] + _SH_C3[1] * xy * z * c[:, 10]
+             + _SH_C3[2] * y * (4 * zz - xx - yy) * c[:, 11] + _SH_C3[3] * z * (2 * zz - 3 * xx - 3 * yy) * c[:, 12]
+             + _SH_C3[4] * x * (4 * zz - xx - yy) * c[:, 13] + _SH_C3[5] * z * (xx - yy) * c[:, 14]
+             + _SH_C3[6] * x * (xx - 3 * yy) * c[:, 15])
+    return (r + 0.5).clamp_min(0.0)
+
+
+def _centroid_dists(verts, fl):
+    fv = verts[fl]
+    return (fv - fv.mean(dim=-2, keepdim=True)).norm(dim=-1)           # [F,3]
+
+
+def face_quaternions(verts, faces):
+    """compute_face_quaternions: the frame [n, normalize(v0 - v1), normalize(n x R1)] as a unit quaternion."""
+    fv = verts[faces.long()]
+    nrm = torch.nn.functional.normalize
+    r0 = nrm(p3d_faces_normals(verts, faces), dim=-1)
+    r1 = nrm(fv[:, 0] - fv[:, 1], dim=-1)
+    r2 = nrm(torch.linalg.cross(r0, r1, dim=-1), dim=-1)
+    return nrm(matrix_to_quaternion(torch.stack([r0, r1, r2], -1)), dim=-1)
+
+
+def edited_frosting_attributes(params, ref_verts, faces, cells, inner_dist, outer_dist, verts, campos, sh_degree,
+                               edition_mask=None, thickness_rescaling="median", orig_quats=None,
+                               deformation_threshold=2.0):
+    """One frame of an edited Frosting scene in torch, as the reference computes it with make_editable(
+    use_simple_adapt=True) (frosting_model.py:649-799, :886-898, :1013-1054; blender/frosting_utils.py:519-571;
+    colours :1479-1484 with get_points_rgb :1304-1352).  `ref_verts`: the base vertices make_editable saw; `verts`: this
+    frame's.  Returns means3D, opacities, scales, rotations, colors_precomp ([P + n_bg] rows) and the shell (inner,
+    outer).  The oracle of frosting_b200.edit."""
+    fl = faces.long()
+    V, F = verts.shape[0], fl.shape[0]
+    em = torch.ones(F, dtype=torch.bool, device=verts.device) if edition_mask is None else edition_mask.bool()
+    gem = em[cells]
+    ref_d, cur_d = _centroid_dists(ref_verts, fl), _centroid_dists(verts, fl)
+    if thickness_rescaling == "median":
+        # two Python floats (.item()) in the reference: their quotient is formed in double
+        f = (cur_d[em].median().double() / ref_d[em].median().double()).float()
+        vfac = torch.ones(V, device=verts.device)
+        vfac[fl[em].unique()] = f
+        gfac = f
+    elif thickness_rescaling == "triangle":
+        ff = torch.ones(F, device=verts.device)
+        ff[em] = (cur_d[em].median(dim=-1).values / ref_d[em].median(dim=-1).values).nan_to_num()
+        s = torch.zeros(V, device=verts.device).index_add(0, fl.reshape(-1), ff.repeat_interleave(3))
+        cnt = torch.zeros(V, device=verts.device).index_add(0, fl.reshape(-1), torch.ones(3 * F, device=verts.device))
+        vfac = s / cnt.clamp(min=1)
+        gfac = ff[cells][gem][:, None]
+    else:
+        raise ValueError(f"thickness rescaling method {thickness_rescaling!r} is not recognized")
+    n = p3d_verts_normals(verts, faces)
+    inner = verts + vfac[:, None] * inner_dist[:, None] * n
+    outer = verts + vfac[:, None] * outer_dist[:, None] * n
+    a = frosting_attributes(params, dict(faces=faces, inner=inner, outer=outer, cells=cells))
+    scales = a["scales"].clone()
+    scales[gem] = scales[gem] * gfac
+    q = a["rotations"].clone()
+    fq, rq = face_quaternions(verts, faces), face_quaternions(ref_verts, faces)
+    c = cells[gem]
+    q[gem] = quaternion_multiply(fq[c], quaternion_multiply(quaternion_invert(rq[c]), q[gem]))
+    keep = (cur_d / ref_d).max(dim=-1).values <= deformation_threshold
+    opac = a["opacities"].clone()
+    opac[gem & ~keep[cells]] = 0.0
+    pos, shs = a["means3D"], a["shs"]
+    if "bg_points" in params:
+        b = frosting_background_attributes(params)
+        pos, opac, scales = torch.cat([pos, b["means3D"]]), torch.cat([opac, b["opacities"]]), torch.cat([scales, b["scales"]])
+        q, shs = torch.cat([q, b["rotations"]]), torch.cat([shs, b["shs"]])
+    dirs = torch.nn.functional.normalize(pos - campos.reshape(1, 3), dim=-1)
+    if orig_quats is not None:
+        rot = quaternion_to_matrix(quaternion_multiply(q, quaternion_invert(orig_quats)))
+        dirs = (dirs[:, None] @ rot)[:, 0]
+    colors = sh_colors(shs[:, :(sh_degree + 1) ** 2], dirs, sh_degree)
+    return dict(means3D=pos, opacities=opac, scales=scales, rotations=q, colors_precomp=colors, inner=inner, outer=outer)
+
+
+def deform_base(verts, t=1.0, centre=(0.0, 0.0, 6.0)):
+    """A non-rigid deformation of a sphere's base vertices: a twist about y growing with height, a bend, and an
+    anisotropic stretch -- so that some faces stretch past ratio 2.  `t` scales it (frames of an animation)."""
+    c = verts.new_tensor(centre)
+    p = verts - c
+    ang = 0.15 * t * p[:, 1]
+    ca, sa = torch.cos(ang), torch.sin(ang)
+    x = ca * p[:, 0] + sa * p[:, 2]
+    z = -sa * p[:, 0] + ca * p[:, 2]
+    y = p[:, 1] * (1.0 + 0.8 * t * (p[:, 1] > 1.5).float() * (p[:, 1] - 1.5))
+    x = x * (1.0 + 0.35 * t) + 0.08 * t * p[:, 1] ** 2
+    z = z * (1.0 - 0.25 * t)
+    return torch.stack([x, y, z], -1) + c

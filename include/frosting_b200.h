@@ -283,6 +283,58 @@ int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const fl
                                        const float* d_g_rotations, const float* d_g_shs,
                                        const fb200_frosting_grads* grads, void* stream);
 
+/* Edited / animated scenes, simple adaptation (frosting_model.py:1013-1054 make_editable(use_simple_adapt=True), the
+ * editable branches of :649-799, blender/frosting_utils.py:519-588 render_composited_image).  Per frame the base
+ * vertices move; fb200_frosting_edit_shell rebuilds the shell and the per-face tables from them, and
+ * fb200_frosting_edit_attributes turns the parameter block into rasterizer inputs with COLOURS precomputed from SH at
+ * view directions rotated by R(q' q_orig^-1) (feed them to fb200_forward as d_colors_precomp).  Forward only.
+ *
+ * Reference capture: with d_ref_quats, d_ref_dists and d_ref_median all NULL, fb200_frosting_edit_shell writes the
+ * face quaternions to d_rel_quats, the distances to d_dists and (median method) their median to d_factor[0], keeps
+ * every face and uses factor 1 -- run it once on the reference vertices and keep those three as the references. */
+#define FB200_RESCALE_MEDIAN 0      /* one factor: median of the edited faces' centroid distances over the reference's */
+#define FB200_RESCALE_TRIANGLE 1    /* per face: median of its three distances over the reference's */
+#define FB200_EDIT_SELECT_WORDS 2051
+typedef struct fb200_frosting_edit {
+    int32_t n_verts, n_faces;
+    int32_t rescaling;                    /* FB200_RESCALE_* */
+    int32_t n_edited;                     /* faces with d_edition_mask set (median: >= 1) */
+    float deformation_threshold;          /* an edited face is dropped when max_k(dist_k / ref_dist_k) > threshold */
+    const float* d_base_verts;            /* [V,3] this frame's (deformed) base vertices */
+    const int32_t* d_faces;               /* [F,3] */
+    const float* d_inner_dist;            /* [V] signed shell offsets along the vertex normal */
+    const float* d_outer_dist;            /* [V] */
+    const uint8_t* d_edition_mask;        /* [F] edited faces */
+    const uint8_t* d_verts_edition_mask;  /* [V] vertices of edited faces */
+    const int32_t* d_vf_offsets;          /* [V+1] vertex -> adjacent face CSR (one entry per face corner) */
+    const int32_t* d_vf_faces;            /* [3F] */
+    const float* d_ref_quats;             /* [F,4] reference face quaternions, 16-byte aligned (NULL: capture) */
+    const float* d_ref_dists;             /* [F,3] reference vertex-to-centroid distances */
+    const float* d_ref_median;            /* [1]   median of the edited faces' reference distances (median method) */
+    /* written by fb200_frosting_edit_shell */
+    float* d_dists;                       /* [F,3] */
+    float* d_face_normals;                /* [F,3] area-weighted face normals (vertex-normal terms) */
+    float* d_rel_quats;                   /* [F,4] face_q * ref_q^-1 on edited faces, identity elsewhere; 16-byte aligned */
+    float* d_face_factor;                 /* [F]   triangle factor (1 on unedited faces) */
+    uint8_t* d_face_keep;                 /* [F]   deformation keep flag */
+    float* d_factor;                      /* [2]   median method: the median, the factor */
+    uint32_t* d_select;                   /* [FB200_EDIT_SELECT_WORDS] scratch of the median's radix select */
+    float* d_inner_verts;                 /* [V,3] the frame's shell */
+    float* d_outer_verts;                 /* [V,3] */
+} fb200_frosting_edit;
+
+int fb200_frosting_edit_shell(const fb200_frosting_edit* e, void* stream);
+/* fp: the parameter block whose d_inner_verts / d_outer_verts are e's shell (d_mask, d_radii unused; d_face_visible
+ * optional: culled rows are not written).  Rows P + n_bg, background rows last: d_rotations 16-byte aligned,
+ * d_orig_quats [P+n_bg,4] 16-byte aligned or NULL (directions unrotated), d_colors [P+n_bg,3].
+ * sh_degree <= sqrt(sh_rest + 1) - 1. */
+int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
+                                   const float* d_campos /*[3]*/, const float* d_orig_quats, float* d_means3D,
+                                   float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
+                                   void* stream);
+/* sizeof(fb200_frosting_edit), for binding mirrors */
+size_t fb200_frosting_edit_struct_size(void);
+
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).
  *   d_pred, d_gt [C,H,W]; d_maps [3,C,H,W] scratch kept for backward; d_partials [fb200_loss_partials(C,H,W)];

@@ -1,0 +1,112 @@
+"""One frame of an animated Frosting scene: the CUDA edit path against the torch chain a user runs without it.
+
+    python tools/frosting_edit_bench.py [--n-bg 0 500000] [--iters 10] [--warmup 3] [--rescaling median]
+
+Scene: the C3 frosting layer (2 M mesh-bound Gaussians, ~1 M-face shell, 1920x1080, SH degree 3, ring camera at radius
+6) plus `n_bg` background Gaussians, made editable (simple adaptation, 70 % of the faces edited); every frame bends the
+sphere by a different twist and squash (`scenes.deform_base` at a frame-dependent strength).  Per frame, timed with
+CUDA events, the two routes alternating:
+  (a) `frosting_render_edited` (csrc/frosting_edit.cu: shell + tables, attributes with SH colours; then the rasterizer);
+  (b) `scenes.edited_frosting_attributes` -- the torch restatement of the reference's per-frame chain (shell with
+      pytorch3d-style normals, rotations, rescaling, deformation drop, SH colours in torch at rotated directions) --
+      then the same rasterizer with colors_precomp.  The reference's `.median().item()` host read-backs are not in it.
+Reports the median of `--iters` frames per route, the max image difference and radii agreement between the routes,
+and the card and its power limit.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import frosting_b200 as fb                       # noqa: E402
+from frosting_b200 import rasterizer as R        # noqa: E402
+from frosting_b200 import scenes                 # noqa: E402
+
+
+def power_limit():
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=20)
+        return r.stdout.strip() or "unknown"
+    except Exception:
+        return "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--n-bg", type=int, nargs="+", default=[0, 500_000])
+    ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--n-mesh", type=int, default=2_000_000)
+    ap.add_argument("--rescaling", default="median", choices=["median", "triangle"])
+    args = ap.parse_args()
+    dev = torch.device("cuda:0")
+    W, H = 1920, 1080
+    cam = scenes.ring_cameras(8, W, H, radius=6.0, device=dev)[0]
+    rs = scenes.settings_for(cam, 3, device=dev)
+    result = {"gpu": torch.cuda.get_device_name(dev), "power_limit": power_limit(), "n_mesh": args.n_mesh,
+              "rescaling": args.rescaling, "runs": []}
+    e = torch.Tensor([])
+    for n_bg in args.n_bg:
+        params, mesh = scenes.frosting_layer(args.n_mesh, scenes.make_camera(W, H), 1237,
+                                             n_faces_target=max(1000, args.n_mesh // 2), n_background=n_bg, device=dev)
+        V, F = mesh["verts"].shape[0], mesh["faces"].shape[0]
+        g = torch.Generator().manual_seed(4)
+        inner_dist = (-0.02 * (1 + 0.2 * torch.rand(V, generator=g))).to(dev)
+        outer_dist = (0.02 * (1 + 0.2 * torch.rand(V, generator=g))).to(dev)
+        em = (torch.rand(F, generator=g) < 0.7).to(dev)
+        quats = torch.cat([params["quats"], params["bg_quats"]]) if n_bg else params["quats"]
+        orig = torch.nn.functional.normalize(quats + 0.2 * torch.randn(quats.shape, generator=g).to(dev), dim=-1)
+        edit = fb.FrostingEdit(mesh["verts"], mesh["faces"], mesh["cells"], inner_dist, outer_dist, edition_mask=em,
+                               thickness_rescaling=args.rescaling)
+
+        def route_a(verts):
+            return fb.frosting_render_edited(params, edit, verts, rs, orig_quats=orig)
+
+        def route_b(verts):
+            a = scenes.edited_frosting_attributes(params, mesh["verts"], mesh["faces"], mesh["cells"], inner_dist,
+                                                  outer_dist, verts, rs.campos, 3, edition_mask=em,
+                                                  thickness_rescaling=args.rescaling, orig_quats=orig)
+            color, radii, _, _ = R._launch_forward(a["means3D"], e, a["colors_precomp"], a["opacities"], a["scales"],
+                                                   a["rotations"], e, rs, None)
+            return color, radii
+
+        routes = {"a_frosting_render_edited": route_a, "b_torch_chain_rasterizer": route_b}
+        frame = lambda i: scenes.deform_base(mesh["verts"], 0.4 + 0.05 * (i % 12))
+        times = {name: [] for name in routes}
+        outs = {}
+        with torch.no_grad():
+            for i in range(args.warmup):
+                for name, fn in routes.items():
+                    outs[name] = fn(frame(i))
+            for i in range(args.iters):
+                verts = frame(i)
+                for name, fn in routes.items():
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    outs[name] = fn(verts)
+                    e1.record()
+                    e1.synchronize()
+                    times[name].append(e0.elapsed_time(e1))
+        (ca, ra), (cb, rb) = outs["a_frosting_render_edited"], outs["b_torch_chain_rasterizer"]
+        run = {"n_bg": n_bg, "rendered": int((ra > 0).sum()), "image_max_abs_diff": (ca - cb).abs().max().item(),
+               "image_px_over_1e-4_frac": ((ca - cb).abs() > 1e-4).float().mean().item(),
+               "radii_agree_frac": (ra == rb).float().mean().item()}
+        for name, t in times.items():
+            t = sorted(t)
+            run[name] = {"median_ms": t[len(t) // 2], "min_ms": t[0], "max_ms": t[-1]}
+        run["speedup_b_over_a"] = run["b_torch_chain_rasterizer"]["median_ms"] / run["a_frosting_render_edited"]["median_ms"]
+        result["runs"].append(run)
+        print(json.dumps(run), flush=True)
+        del params, mesh, outs, edit
+        torch.cuda.empty_cache()
+    print(json.dumps(result))
+
+
+if __name__ == "__main__":
+    main()
