@@ -21,6 +21,7 @@ EXPORTED = [
     "fb200_profile_enable", "fb200_profile_read", "fb200_kernel_launches",
     "fb200_frosting_attributes", "fb200_frosting_attributes_backward",
     "fb200_frosting_edit_shell", "fb200_frosting_edit_attributes", "fb200_frosting_edit_struct_size",
+    "fb200_frosting_edit_complex_capture", "fb200_frosting_edit_attributes_complex",
     "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
@@ -180,6 +181,12 @@ def lib():
         [C.c_void_p] * 8
     L.fb200_frosting_edit_attributes.restype = C.c_int
     L.fb200_frosting_edit_struct_size.restype = C.c_size_t
+    L.fb200_frosting_edit_complex_capture.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams)] + \
+        [C.c_void_p] * 4
+    L.fb200_frosting_edit_complex_capture.restype = C.c_int
+    L.fb200_frosting_edit_attributes_complex.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams),
+                                                         C.c_int32] + [C.c_void_p] * 10
+    L.fb200_frosting_edit_attributes_complex.restype = C.c_int
     L.fb200_loss_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.fb200_loss_partials.restype = C.c_size_t
     L.fb200_l1_dssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,

@@ -531,10 +531,9 @@ int fb200_frosting_edit_shell(const fb200_frosting_edit* e, void* stream) {
     return check(launch_frosting_edit_shell(*e, static_cast<cudaStream_t>(stream)), "frosting_edit_shell");
 }
 
-int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
-                                   const float* d_campos, const float* d_orig_quats, float* d_means3D,
-                                   float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
-                                   void* stream) {
+static int check_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
+                                 const float* d_campos, const float* d_orig_quats, float* d_means3D,
+                                 float* d_opacities, float* d_scales, float* d_rotations, float* d_colors) {
     int rc = check_edit(e);
     if (rc != FB200_OK) return rc;
     if ((rc = check_frosting(fp)) != FB200_OK) return rc;
@@ -547,9 +546,56 @@ int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_fro
         return fail(FB200_EINVAL, "frosting_edit: missing output pointer%s");
     if ((reinterpret_cast<uintptr_t>(d_rotations) & 15) || (reinterpret_cast<uintptr_t>(d_orig_quats) & 15))
         return fail(FB200_EINVAL, "frosting_edit: rotations / orig quats must be 16-byte aligned%s");
+    return FB200_OK;
+}
+
+int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
+                                   const float* d_campos, const float* d_orig_quats, float* d_means3D,
+                                   float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
+                                   void* stream) {
+    const int rc = check_edit_attributes(e, fp, sh_degree, d_campos, d_orig_quats, d_means3D, d_opacities, d_scales,
+                                         d_rotations, d_colors);
+    if (rc != FB200_OK) return rc;
     return check(launch_frosting_edit_attr(*e, *fp, sh_degree, d_campos, d_orig_quats, d_means3D, d_opacities, d_scales,
                                            d_rotations, d_colors, static_cast<cudaStream_t>(stream)),
                  "frosting_edit_attributes");
+}
+
+// the complex adaptation's tables: [F,9] cell transforms when a face is edited, [P,9] canonical transforms
+static int check_edit_complex(const fb200_frosting_edit* e, const fb200_frosting_params* fp, const float* d_cell_T,
+                              const float* d_canonical) {
+    if (e->n_edited > 0 && !d_cell_T) return fail(FB200_EINVAL, "frosting_edit_complex: missing cell transforms%s");
+    if (fp->P > 0 && !d_canonical) return fail(FB200_EINVAL, "frosting_edit_complex: missing canonical transforms%s");
+    return FB200_OK;
+}
+
+int fb200_frosting_edit_complex_capture(const fb200_frosting_edit* e, const fb200_frosting_params* fp, float* d_cell_T,
+                                        float* d_canonical, uint32_t* d_n_singular, void* stream) {
+    int rc = check_edit(e);
+    if (rc != FB200_OK) return rc;
+    if ((rc = check_frosting(fp)) != FB200_OK) return rc;
+    if (fp->n_faces != e->n_faces || fp->n_verts != e->n_verts)
+        return fail(FB200_EINVAL, "frosting_edit: the parameter block's mesh does not match the edit's%s");
+    if ((rc = check_edit_complex(e, fp, d_cell_T, d_canonical)) != FB200_OK) return rc;
+    if (!d_n_singular) return fail(FB200_EINVAL, "frosting_edit_complex: missing singular-cell counter%s");
+    return check(launch_frosting_edit_complex_capture(*e, *fp, d_cell_T, d_canonical, d_n_singular,
+                                                      static_cast<cudaStream_t>(stream)),
+                 "frosting_edit_complex_capture");
+}
+
+int fb200_frosting_edit_attributes_complex(const fb200_frosting_edit* e, const fb200_frosting_params* fp,
+                                           int32_t sh_degree, const float* d_campos, const float* d_orig_quats,
+                                           const float* d_canonical, float* d_cell_T, float* d_means3D,
+                                           float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
+                                           void* stream) {
+    int rc = check_edit_attributes(e, fp, sh_degree, d_campos, d_orig_quats, d_means3D, d_opacities, d_scales,
+                                   d_rotations, d_colors);
+    if (rc != FB200_OK) return rc;
+    if ((rc = check_edit_complex(e, fp, d_cell_T, d_canonical)) != FB200_OK) return rc;
+    return check(launch_frosting_edit_attr_complex(*e, *fp, sh_degree, d_campos, d_orig_quats, d_canonical, d_cell_T,
+                                                   d_means3D, d_opacities, d_scales, d_rotations, d_colors,
+                                                   static_cast<cudaStream_t>(stream)),
+                 "frosting_edit_attributes_complex");
 }
 
 size_t fb200_loss_partials(int32_t C, int32_t H, int32_t W) {

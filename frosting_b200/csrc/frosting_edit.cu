@@ -1,4 +1,5 @@
-// frosting_edit.cu -- per-frame attributes of an EDITED / ANIMATED Frosting scene, simple adaptation (SURVEY.md row a21).
+// frosting_edit.cu -- per-frame attributes of an EDITED / ANIMATED Frosting scene (SURVEY.md row a21), simple and
+// complex adaptation.
 //
 // Replaces the torch chain Frosting runs on every frame of a deformed base mesh (render_blender_scene.py ->
 // blender/frosting_utils.py:551-588 render_composited_image, with make_editable(use_simple_adapt=True)):
@@ -19,6 +20,10 @@
 //                atomics: frames are reproducible bit for bit), thickness factor, inner / outer shell vertices;
 //   attributes   one thread per Gaussian (mesh rows, then background rows): position in the new shell, sigmoid
 //                opacity (0 on dropped faces), exp scale * factor, rotated quaternion, SH colour.
+// The complex adaptation (make_editable(use_simple_adapt=False), frosting_model.py:900-967, :1055-1119, :1149-1183) adds
+//   cell pass    one thread per edited face: the cell transform T (after the shell passes: the median is on the device);
+//   capture      once, one thread per mesh Gaussian: the canonical transform C = T_ref[cell]^-1 R(q) diag(exp s);
+// and an attribute-kernel instance whose edited rows take scales and rotation from M = T_frame[cell] C.
 // pytorch3d's maths (Meshes normals, matrix_to_quaternion, quaternion_multiply / invert / to_matrix) is restated from
 // its documented definitions; see DESIGN.md.
 #include <cfloat>
@@ -237,6 +242,159 @@ edit_vertex_kernel(fb200_frosting_edit e) {
     e.d_outer_verts[3 * v + 2] = fadd(b.z, fmul(dout, n.z));
 }
 
+// ---- complex adaptation: cell transforms, canonical transforms ----
+// axis_bary_shifts of compute_cell_transformations: float64 constants rounded to fp32, as torch.tensor(..., float32) does
+constexpr float kShiftA = (float)(1.4142135623730951 / 2.0);          // np.sqrt(2) / 2
+constexpr float kShiftB = (float)(1.0 / 2.449489742783178);           // 1 / np.sqrt(6)
+constexpr float kShiftB2 = (float)(2.0 / 2.449489742783178);          // 2 / np.sqrt(6)
+
+__device__ __forceinline__ V3 scale3(V3 a, float s) { return {fmul(a.x, s), fmul(a.y, s), fmul(a.z, s)}; }
+__device__ __forceinline__ float dot3(V3 a, V3 b) { return fadd(fadd(fmul(a.x, b.x), fmul(a.y, b.y)), fmul(a.z, b.z)); }
+__device__ __forceinline__ bool is_zero3(V3 a) { return a.x == 0.f && a.y == 0.f && a.z == 0.f; }
+
+// compute_cell_transformations(faces_mask=edition_mask), one thread per face: T = [a', b', normalize(n) * d] (columns,
+// row-major T[3r + c]) on edited faces.  a, b: the axis_bary_shifts products summed in v0, v1, v2 order; the shorter one
+// Gram-Schmidt-orthogonalised against the longer as written at :943-946, both in their own slots.  d: the median of the
+// edited faces' distances (median method, d_factor[0]) or the face's own median distance, 0 -> 1 (triangle).  capture:
+// make_editable's fix-up of singular cells -- a zero column 0 becomes c1 x c2, then a zero column 1 becomes c2 x c0 (a
+// zero column is the only way torch.det is exactly 0 that the fix-up changes)
+__global__ void __launch_bounds__(kEditThreads)
+edit_cell_kernel(fb200_frosting_edit e, float* cell_T, int capture) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= e.n_faces || __ldg(e.d_edition_mask + f) == 0) return;
+    V3 v[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) v[k] = ld3(e.d_base_verts + 3 * (size_t)__ldg(e.d_faces + 3 * f + k));
+    V3 a, b;
+    a.x = fadd(fadd(fmul(-kShiftA, v[0].x), fmul(kShiftA, v[1].x)), fmul(0.f, v[2].x));
+    a.y = fadd(fadd(fmul(-kShiftA, v[0].y), fmul(kShiftA, v[1].y)), fmul(0.f, v[2].y));
+    a.z = fadd(fadd(fmul(-kShiftA, v[0].z), fmul(kShiftA, v[1].z)), fmul(0.f, v[2].z));
+    b.x = fadd(fadd(fmul(-kShiftB, v[0].x), fmul(-kShiftB, v[1].x)), fmul(kShiftB2, v[2].x));
+    b.y = fadd(fadd(fmul(-kShiftB, v[0].y), fmul(-kShiftB, v[1].y)), fmul(kShiftB2, v[2].y));
+    b.z = fadd(fadd(fmul(-kShiftB, v[0].z), fmul(-kShiftB, v[1].z)), fmul(kShiftB2, v[2].z));
+    const bool swap = norm3(b) > norm3(a);                // the longer axis first; a first on ties
+    const V3 first = swap ? b : a, second = swap ? a : b;
+    const float dt = dot3(second, first), sq = dot3(first, first);
+    const V3 ortho = {fadd(second.x, -__fdiv_rn(fmul(dt, first.x), sq)), fadd(second.y, -__fdiv_rn(fmul(dt, first.y), sq)),
+                      fadd(second.z, -__fdiv_rn(fmul(dt, first.z), sq))};
+    V3 c0 = swap ? ortho : first, c1 = swap ? first : ortho;
+    float d;
+    if (e.rescaling == FB200_RESCALE_MEDIAN) {
+        d = e.d_factor[0];
+    } else {
+        d = median3(e.d_dists[3 * f], e.d_dists[3 * f + 1], e.d_dists[3 * f + 2]);
+        if (d == 0.f) d = 1.0f;
+    }
+    const V3 n = normalize_eps(normalize_eps(cross(sub(v[1], v[0]), sub(v[2], v[0])), 1e-6f), 1e-12f);
+    const V3 c2 = scale3(n, d);
+    if (capture) {
+        if (is_zero3(c0)) c0 = cross(c1, c2);
+        if (is_zero3(c1)) c1 = cross(c2, c0);
+    }
+    float* T = cell_T + 9 * (size_t)f;
+    T[0] = c0.x; T[1] = c1.x; T[2] = c2.x;
+    T[3] = c0.y; T[4] = c1.y; T[5] = c2.y;
+    T[6] = c0.z; T[7] = c1.z; T[8] = c2.z;
+}
+
+__device__ __forceinline__ void swap_rows(float* m, int r0, int r1) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { const float t = m[3 * r0 + c]; m[3 * r0 + c] = m[3 * r1 + c]; m[3 * r1 + c] = t; }
+}
+
+// make_editable(use_simple_adapt=False), one thread per mesh Gaussian: C = T_ref[cell]^-1 G, G = R(normalize(q)) diag(exp(s)),
+// by a 3x3 LU with partial pivoting (getrf's rule: the first largest |a|), then getrs' two triangular solves.  An exact
+// zero pivot is a singular cell (torch.linalg.solve raises): the Gaussian is counted into n_singular, its C set to zero.
+// Unedited rows get C = 0.
+__global__ void __launch_bounds__(kEditThreads)
+edit_capture_kernel(fb200_frosting_edit e, fb200_frosting_params p, const float* cell_T, float* canonical,
+                    uint32_t* n_singular) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= p.P) return;
+    const size_t i = (size_t)idx;
+    float* out = canonical + 9 * i;
+    const long long cell = __ldg(p.d_cells + i);
+    if (__ldg(e.d_edition_mask + cell) == 0) {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) out[k] = 0.f;
+        return;
+    }
+    float nrm;
+    const float4 q = frost_normalize(__ldg(reinterpret_cast<const float4*>(p.d_quats) + i), nrm);
+    float B[9], A[9];
+    q_to_matrix(q, B);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float s = expf(__ldg(p.d_log_scales + 3 * i + c));
+#pragma unroll
+        for (int r = 0; r < 3; ++r) B[3 * r + c] = fmul(B[3 * r + c], s);
+    }
+#pragma unroll
+    for (int k = 0; k < 9; ++k) A[k] = __ldg(cell_T + 9 * (size_t)cell + k);
+    bool singular = false;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        int piv = j;
+#pragma unroll
+        for (int r = j + 1; r < 3; ++r) if (fabsf(A[3 * r + j]) > fabsf(A[3 * piv + j])) piv = r;
+        if (piv == 1) { swap_rows(A, j, 1); swap_rows(B, j, 1); }
+        else if (piv == 2) { swap_rows(A, j, 2); swap_rows(B, j, 2); }
+        if (A[3 * j + j] == 0.f) { singular = true; continue; }
+#pragma unroll
+        for (int r = j + 1; r < 3; ++r) {
+            const float l = __fdiv_rn(A[3 * r + j], A[3 * j + j]);
+            A[3 * r + j] = l;
+#pragma unroll
+            for (int c = j + 1; c < 3; ++c) A[3 * r + c] = fadd(A[3 * r + c], -fmul(l, A[3 * j + c]));
+        }
+    }
+    if (singular) {
+        atomicAdd(n_singular, 1u);
+#pragma unroll
+        for (int k = 0; k < 9; ++k) out[k] = 0.f;
+        return;
+    }
+    // L (unit lower) then U, column by column of B as trsm does
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+            for (int r = k + 1; r < 3; ++r) B[3 * r + c] = fadd(B[3 * r + c], -fmul(B[3 * k + c], A[3 * r + k]));
+#pragma unroll
+        for (int k = 2; k >= 0; --k) {
+            B[3 * k + c] = __fdiv_rn(B[3 * k + c], A[3 * k + k]);
+#pragma unroll
+            for (int r = 0; r < k; ++r) B[3 * r + c] = fadd(B[3 * r + c], -fmul(B[3 * k + c], A[3 * r + k]));
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 9; ++k) out[k] = B[k];
+}
+
+// get_edited_quaternions_and_scales for one edited Gaussian: M = T_frame[cell] C, scales = column norms (nan_to_num),
+// q = normalize(matrix_to_quaternion(M / max(scales, 1e-10)))
+__device__ __forceinline__ float4 complex_edit(const float* T, const float* Cm, float* scales) {
+    float t[9], c[9], m[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) { t[k] = __ldg(T + k); c[k] = __ldg(Cm + k); }
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int col = 0; col < 3; ++col)
+            m[3 * r + col] = fadd(fadd(fmul(t[3 * r], c[col]), fmul(t[3 * r + 1], c[3 + col])), fmul(t[3 * r + 2], c[6 + col]));
+#pragma unroll
+    for (int col = 0; col < 3; ++col) {
+        const float s = norm3({m[col], m[3 + col], m[6 + col]});
+        scales[col] = nan_to_num(s);
+        const float dv = fmaxf(s, 1e-10f);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) m[3 * r + col] = __fdiv_rn(m[3 * r + col], dv);
+    }
+    float nrm;
+    return frost_normalize(matrix_to_q(m), nrm);
+}
+
 // ---- per-Gaussian attributes ----
 struct EditAttrArgs {
     fb200_frosting_edit e;
@@ -245,8 +403,13 @@ struct EditAttrArgs {
     const float* campos;
     const float* orig_quats;       // [P + n_bg, 4] or NULL
     float* means3D; float* opacities; float* scales; float* rotations; float* colors;
+    const float* cell_T;           // complex adaptation: [F,9] this frame's cell transforms
+    const float* canonical;        // complex adaptation: [P,9] canonical transforms
 };
 
+// Complex = false: the simple adaptation (rotate by the face's relative rotation, rescale by the thickness factor);
+// true: edited rows from T_frame[cell] C[i], and every mesh row's NaN quaternion -> identity, scales nan_to_num'd
+template <bool Complex>
 __global__ void __launch_bounds__(kEditThreads)
 edit_attr_kernel(EditAttrArgs a) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -271,17 +434,26 @@ edit_attr_kernel(EditAttrArgs a) {
     const bool edited = !bg && __ldg(a.e.d_edition_mask + cell) != 0;
     float opacity = frost_sigmoid(__ldg(src.opacity_logits));
     if (edited && a.e.d_face_keep[cell] == 0) opacity = 0.f;
+    float4 q;
+    float sc[3];
     float factor = 1.0f;
-    if (edited) factor = a.e.rescaling == FB200_RESCALE_MEDIAN ? a.e.d_factor[1] : a.e.d_face_factor[cell];
-    float nrm;
-    float4 q = frost_normalize(__ldg(reinterpret_cast<const float4*>(src.quats)), nrm);
-    if (edited) q = q_mul(reinterpret_cast<const float4*>(a.e.d_rel_quats)[cell], q);
+    if (Complex && edited) {
+        q = complex_edit(a.cell_T + 9 * cell, a.canonical + 9 * i, sc);
+    } else {
+        if (edited) factor = a.e.rescaling == FB200_RESCALE_MEDIAN ? a.e.d_factor[1] : a.e.d_face_factor[cell];
+        float nrm;
+        q = frost_normalize(__ldg(reinterpret_cast<const float4*>(src.quats)), nrm);
+        if (edited) q = q_mul(reinterpret_cast<const float4*>(a.e.d_rel_quats)[cell], q);
+    }
+    if (Complex && !bg && (isnan(q.x) || isnan(q.y) || isnan(q.z) || isnan(q.w))) q = make_float4(1.f, 0.f, 0.f, 0.f);
     a.means3D[3 * i] = px; a.means3D[3 * i + 1] = py; a.means3D[3 * i + 2] = pz;
     a.opacities[i] = opacity;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
+        if (Complex && edited) { a.scales[3 * i + k] = sc[k]; continue; }
         const float s = expf(__ldg(src.log_scales + k));
-        a.scales[3 * i + k] = edited ? fmul(s, factor) : s;
+        // complex: the reference nan_to_num's every mesh row's scale
+        a.scales[3 * i + k] = Complex ? (bg ? s : nan_to_num(s)) : edited ? fmul(s, factor) : s;
     }
     reinterpret_cast<float4*>(a.rotations)[i] = q;
     // colour: SH at the view direction, rotated into the Gaussian's original frame (row vector times R)
@@ -331,18 +503,63 @@ cudaError_t launch_frosting_edit_shell(const fb200_frosting_edit& e, cudaStream_
     return cudaGetLastError();
 }
 
-cudaError_t launch_frosting_edit_attr(const fb200_frosting_edit& e, const fb200_frosting_params& p, int sh_degree,
-                                      const float* campos, const float* orig_quats, float* means3D, float* opacities,
-                                      float* scales, float* rotations, float* colors, cudaStream_t s) {
+namespace {
+
+void launch_cells(const fb200_frosting_edit& e, float* cell_T, int capture, cudaStream_t s) {
+    if (e.n_faces > 0 && e.n_edited > 0) {
+        edit_cell_kernel<<<(e.n_faces + kEditThreads - 1) / kEditThreads, kEditThreads, 0, s>>>(e, cell_T, capture);
+        count_launch();
+    }
+}
+
+cudaError_t launch_attr(bool complex, const fb200_frosting_edit& e, const fb200_frosting_params& p, int sh_degree,
+                        const float* campos, const float* orig_quats, const float* canonical, const float* cell_T,
+                        float* means3D, float* opacities, float* scales, float* rotations, float* colors,
+                        cudaStream_t s) {
     const int rows = p.P + p.n_bg;
     if (rows > 0) {
         EditAttrArgs a;
         a.e = e; a.p = p; a.sh_degree = sh_degree; a.campos = campos; a.orig_quats = orig_quats;
         a.means3D = means3D; a.opacities = opacities; a.scales = scales; a.rotations = rotations; a.colors = colors;
-        edit_attr_kernel<<<(rows + kEditThreads - 1) / kEditThreads, kEditThreads, 0, s>>>(a);
+        a.cell_T = cell_T; a.canonical = canonical;
+        const auto kernel = complex ? edit_attr_kernel<true> : edit_attr_kernel<false>;
+        kernel<<<(rows + kEditThreads - 1) / kEditThreads, kEditThreads, 0, s>>>(a);
         count_launch();
     }
     return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_frosting_edit_attr(const fb200_frosting_edit& e, const fb200_frosting_params& p, int sh_degree,
+                                      const float* campos, const float* orig_quats, float* means3D, float* opacities,
+                                      float* scales, float* rotations, float* colors, cudaStream_t s) {
+    return launch_attr(false, e, p, sh_degree, campos, orig_quats, nullptr, nullptr, means3D, opacities, scales, rotations,
+                       colors, s);
+}
+
+cudaError_t launch_frosting_edit_complex_capture(const fb200_frosting_edit& e, const fb200_frosting_params& p,
+                                                 float* cell_T, float* canonical, uint32_t* n_singular,
+                                                 cudaStream_t s) {
+    cudaError_t err = cudaMemsetAsync(n_singular, 0, sizeof(uint32_t), s);
+    if (err != cudaSuccess) return err;
+    launch_cells(e, cell_T, 1, s);
+    if (p.P > 0) {
+        edit_capture_kernel<<<(p.P + kEditThreads - 1) / kEditThreads, kEditThreads, 0, s>>>(e, p, cell_T, canonical,
+                                                                                              n_singular);
+        count_launch();
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_frosting_edit_attr_complex(const fb200_frosting_edit& e, const fb200_frosting_params& p,
+                                              int sh_degree, const float* campos, const float* orig_quats,
+                                              const float* canonical, float* cell_T, float* means3D,
+                                              float* opacities, float* scales, float* rotations, float* colors,
+                                              cudaStream_t s) {
+    launch_cells(e, cell_T, 0, s);
+    return launch_attr(true, e, p, sh_degree, campos, orig_quats, canonical, cell_T, means3D, opacities, scales, rotations,
+                       colors, s);
 }
 
 }  // namespace fb200

@@ -11,7 +11,8 @@ several host read-backs per frame in the reference.  Here:
     image, radii = frosting_render_edited(params, edit, frame_base_verts, raster_settings, orig_quats=...)
 
 is two CUDA calls (csrc/frosting_edit.cu: shell + tables, then the per-Gaussian attributes) and the existing rasterizer
-forward with precomputed colours.  Forward only, simple adaptation only.
+forward with precomputed colours.  The complex adaptation (`make_editable(use_simple_adapt=False)`, per-Gaussian
+canonical transforms) is `FrostingEditComplex(params, ref_base_verts, faces, ...)`, used the same way.  Forward only.
 """
 import ctypes as C
 
@@ -34,8 +35,8 @@ class FrostingEdit:
     def __init__(self, base_verts, faces, cells, inner_dist, outer_dist, edition_mask=None, thickness_rescaling="median",
                  adaptation="simple"):
         if adaptation != "simple":
-            raise NotImplementedError(f"adaptation {adaptation!r}: only the simple adaptation (use_simple_adapt=True) is "
-                                      "implemented; the complex one (per-Gaussian canonical transforms) is not")
+            raise NotImplementedError(f"adaptation {adaptation!r}: FrostingEdit is the simple adaptation "
+                                      "(use_simple_adapt=True); the complex one is FrostingEditComplex")
         if thickness_rescaling not in RESCALING:
             raise ValueError(f"thickness rescaling method {thickness_rescaling!r} is not recognized "
                              f"(one of {sorted(RESCALING)})")
@@ -74,10 +75,15 @@ class FrostingEdit:
         self.factor = torch.ones((2,), **o)
         self._select = torch.empty((_lib.EDIT_SELECT_WORDS,), dtype=torch.int32, device=dev)
         self.ref_quats = self.ref_dists = self.ref_median = None
-        # reference capture: the same kernels over the reference vertices, so an unedited frame reproduces them bit for bit
-        self._shell(f32(base_verts, "base_verts"), 2.0)
+        self._capture(f32(base_verts, "base_verts"))
+
+    def _capture(self, base_verts):
+        """Reference capture: the same kernels over the reference vertices, so an unedited frame reproduces them bit for
+        bit.  Returns the capture's struct and shell."""
+        st, inner, outer = self._shell(base_verts, 2.0)
         self.ref_quats, self.ref_dists = self.rel_quats.clone(), self.dists.clone()
-        self.ref_median = self.factor[:1].clone() if thickness_rescaling == "median" else None
+        self.ref_median = self.factor[:1].clone() if self.rescaling == "median" else None
+        return st, inner, outer
 
     def _struct(self, base_verts, threshold, inner, outer):
         return _lib.FrostingEdit(
@@ -105,6 +111,18 @@ class FrostingEdit:
         _, inner, outer = self._shell(R._f32c(base_verts, self.device, "base_verts"), deformation_threshold)
         return inner, outer
 
+    def _block(self, params, inner, outer, face_visible):
+        fp, keep, _, dev = _params_block(params["bary_logits"], params["opacity_logits"], params["log_scales"],
+                                         params["quats"], params["sh_dc"], params["sh_rest"], inner, outer, self.cells,
+                                         self.faces, face_visible, background_params(params))
+        if fp.P != self.cells.numel():
+            raise ValueError("params have a different number of mesh-bound Gaussians than the edit's cells")
+        return fp, keep, dev
+
+    def _launch_attributes(self, st, fp, sh_degree, cp, oq, outs, stream):
+        _lib.check(_lib.lib().fb200_frosting_edit_attributes(C.byref(st), C.byref(fp), int(sh_degree), _p(cp), _p(oq),
+                                                              *(_p(t) for t in outs), stream))
+
     @torch.no_grad()
     def attributes(self, params, base_verts, campos, sh_degree, orig_quats=None, deformation_threshold=2.0,
                    face_visible=None):
@@ -115,12 +133,7 @@ class FrostingEdit:
         culled faces are skipped (zero rows)."""
         base_verts = R._f32c(base_verts, self.device, "base_verts")
         st, inner, outer = self._shell(base_verts, deformation_threshold)
-        bg = background_params(params)
-        fp, keep, _, dev = _params_block(params["bary_logits"], params["opacity_logits"], params["log_scales"],
-                                         params["quats"], params["sh_dc"], params["sh_rest"], inner, outer, self.cells,
-                                         self.faces, face_visible, bg)
-        if fp.P != self.cells.numel():
-            raise ValueError("params have a different number of mesh-bound Gaussians than the edit's cells")
+        fp, keep, dev = self._block(params, inner, outer, face_visible)
         rows = fp.P + fp.n_bg
         oq = None
         if orig_quats is not None:
@@ -133,12 +146,52 @@ class FrostingEdit:
         means3D, opac, scales = alloc((rows, 3), **o), alloc((rows, 1), **o), alloc((rows, 3), **o)
         rots, colors = alloc((rows, 4), **o), alloc((rows, 3), **o)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().fb200_frosting_edit_attributes(
-                C.byref(st), C.byref(fp), int(sh_degree), _p(cp), _p(oq), _p(means3D), _p(opac), _p(scales),
-                _p(rots), _p(colors), _stream(dev)))
+            self._launch_attributes(st, fp, sh_degree, cp, oq, (means3D, opac, scales, rots, colors), _stream(dev))
         del keep
         return dict(means3D=means3D, opacities=opac, scales=scales, rotations=rots, colors_precomp=colors,
                     inner=inner, outer=outer)
+
+
+class FrostingEditComplex(FrostingEdit):
+    """The reference state of `make_editable(use_simple_adapt=False, edition_mask, thickness_rescaling_method)` -- the
+    complex adaptation, the default of make_editable and of Frosting's Blender pipeline.  On top of FrostingEdit's
+    capture, each edited Gaussian keeps a canonical transform C = T_ref[cell]^-1 R(q) diag(exp(s)) from the `params`
+    given here (`quats`, `log_scales`), where T maps a canonical cell to the world (two orthogonalised in-plane axes and
+    the normal scaled by the median distance).  Per frame the scales are the column norms of T_frame[cell] C and the
+    rotation is that matrix's; shell, positions, opacities, background rows and colours follow the simple path.
+    `cell_T` [F,3,3] (the last frame's, edited faces) and `canonical` [P,3,3] (0 on unedited rows) stay readable.
+    Raises ValueError when an edited Gaussian's reference cell is singular (a degenerate edited face), as the
+    reference's solve does.  Rebuild it when the Gaussians' rotations or scales change."""
+
+    def __init__(self, params, base_verts, faces, cells, inner_dist, outer_dist, edition_mask=None,
+                 thickness_rescaling="median"):
+        self._capture_params = params
+        super().__init__(base_verts, faces, cells, inner_dist, outer_dist, edition_mask=edition_mask,
+                         thickness_rescaling=thickness_rescaling)
+        del self._capture_params
+
+    def _capture(self, base_verts):
+        # after the reference shell, d_dists / d_factor[0] hold the reference distances and median the cells scale by
+        st, inner, outer = super()._capture(base_verts)
+        fp, keep, dev = self._block(self._capture_params, inner, outer, None)
+        o = dict(dtype=torch.float32, device=dev)
+        self.cell_T = torch.zeros((self.n_faces, 3, 3), **o)
+        self.canonical = torch.empty((fp.P, 3, 3), **o)
+        n_singular = torch.empty((1,), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().fb200_frosting_edit_complex_capture(
+                C.byref(st), C.byref(fp), _p(self.cell_T), _p(self.canonical), _p(n_singular), _stream(dev)))
+        del keep
+        n = int(n_singular.item())                      # the one host read-back, at capture only
+        if n:
+            raise ValueError(f"{n} edited Gaussian(s) sit on faces whose cell transformation is singular even after "
+                             "the fix-up (degenerate edited faces): their canonical transforms are undefined")
+        return st, inner, outer
+
+    def _launch_attributes(self, st, fp, sh_degree, cp, oq, outs, stream):
+        _lib.check(_lib.lib().fb200_frosting_edit_attributes_complex(
+            C.byref(st), C.byref(fp), int(sh_degree), _p(cp), _p(oq), _p(self.canonical), _p(self.cell_T),
+            *(_p(t) for t in outs), stream))
 
 
 @torch.no_grad()

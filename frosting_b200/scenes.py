@@ -362,14 +362,75 @@ def face_quaternions(verts, faces):
     return nrm(matrix_to_quaternion(torch.stack([r0, r1, r2], -1)), dim=-1)
 
 
+def cell_transformations(verts, faces, edition_mask=None, thickness_rescaling="median", fix_singular=False):
+    """compute_cell_transformations(faces_mask=edition_mask) (frosting_model.py:900-967): [F,3,3] transforms from the
+    canonical cell to the world, columns [a', b', normalize(n) * d] -- the axis_bary_shifts axes a, b with the shorter
+    Gram-Schmidt-orthogonalised against the longer, each in its own slot; d the median of the edited faces' centroid
+    distances (median) or the face's own median distance, 0 -> 1 (triangle).  Zero on unedited faces.
+    `fix_singular`: make_editable's fix-up where det(T) == 0 (:1073-1112): a zero column 0 becomes c1 x c2, then a zero
+    column 1 becomes c2 x c0."""
+    fl = faces.long()
+    F = fl.shape[0]
+    em = torch.ones(F, dtype=torch.bool, device=verts.device) if edition_mask is None else edition_mask.bool()
+    fv = verts[fl]
+    r2, r6 = math.sqrt(2), math.sqrt(6)
+    shifts = torch.tensor([[-r2 / 2, r2 / 2, 0.0], [-1 / r6, -1 / r6, 2 / r6]], dtype=torch.float32, device=verts.device)
+    ax = (shifts[None, :, :, None] * fv[:, None]).sum(dim=-2)          # [F,2,3]: v0, v1, v2 terms summed in order
+    d_all = _centroid_dists(verts, fl)
+    if thickness_rescaling == "median":
+        d = d_all[em].median()
+    elif thickness_rescaling == "triangle":
+        d = torch.ones(F, device=verts.device)
+        d[em] = d_all[em].median(dim=-1).values
+        d = torch.where(d == 0, torch.ones_like(d), d)[:, None]
+    else:
+        raise ValueError(f"thickness rescaling method {thickness_rescaling!r} is not recognized")
+    n = torch.nn.functional.normalize(p3d_faces_normals(verts, faces), dim=-1) * d
+    a, b = ax[:, 0], ax[:, 1]
+    swap = (b.norm(dim=-1) > a.norm(dim=-1))[:, None]                   # the longer axis first; a first on ties
+    first, second = torch.where(swap, b, a), torch.where(swap, a, b)
+    ortho = second - ((second * first).sum(dim=-1, keepdim=True) * first / (first ** 2).sum(dim=-1, keepdim=True))
+    T = torch.stack([torch.where(swap, ortho, first), torch.where(swap, first, ortho), n], -1)
+    T = torch.where(em[:, None, None], T, torch.zeros_like(T))
+    if fix_singular:
+        sing = em & (torch.linalg.det(T) == 0)
+        if bool(sing.any()):
+            t = T[sing]
+            z0 = (t[..., 0] == 0).all(dim=-1)
+            t[z0, :, 0] = torch.linalg.cross(t[z0, :, 1], t[z0, :, 2], dim=-1)
+            z1 = (t[..., 1] == 0).all(dim=-1)
+            t[z1, :, 1] = torch.linalg.cross(t[z1, :, 2], t[z1, :, 0], dim=-1)
+            T[sing] = t
+    return T
+
+
+def complex_canonical_transforms(params, ref_verts, faces, cells, edition_mask=None, thickness_rescaling="median"):
+    """make_editable(use_simple_adapt=False) (frosting_model.py:1055-1119): the canonical transforms
+    C = T_ref[cell]^-1 R(normalize(q)) diag(exp(s)) of the edited Gaussians, [P,3,3] with zeros on unedited rows, and
+    T_ref.  torch.linalg.solve raises where an edited Gaussian's cell stays singular, as the reference does."""
+    F = faces.shape[0]
+    em = torch.ones(F, dtype=torch.bool, device=ref_verts.device) if edition_mask is None else edition_mask.bool()
+    gem = em[cells]
+    T_ref = cell_transformations(ref_verts, faces, em, thickness_rescaling, fix_singular=True)
+    G = quaternion_to_matrix(torch.nn.functional.normalize(params["quats"][gem], dim=-1))
+    G = G * torch.exp(params["log_scales"][gem])[..., None, :]
+    C = torch.zeros((cells.shape[0], 3, 3), dtype=G.dtype, device=G.device)
+    C[gem] = torch.linalg.solve(T_ref[cells[gem]], G)
+    return C, T_ref
+
+
 def edited_frosting_attributes(params, ref_verts, faces, cells, inner_dist, outer_dist, verts, campos, sh_degree,
                                edition_mask=None, thickness_rescaling="median", orig_quats=None,
-                               deformation_threshold=2.0):
+                               deformation_threshold=2.0, adaptation="simple", canonical=None):
     """One frame of an edited Frosting scene in torch, as the reference computes it with make_editable(
     use_simple_adapt=True) (frosting_model.py:649-799, :886-898, :1013-1054; blender/frosting_utils.py:519-571;
     colours :1479-1484 with get_points_rgb :1304-1352).  `ref_verts`: the base vertices make_editable saw; `verts`: this
     frame's.  Returns means3D, opacities, scales, rotations, colors_precomp ([P + n_bg] rows) and the shell (inner,
-    outer).  The oracle of frosting_b200.edit."""
+    outer).  The oracle of frosting_b200.edit.
+    `adaptation="complex"`: make_editable(use_simple_adapt=False) -- edited rows from M = T_frame[cell] C
+    (get_edited_quaternions_and_scales, :1149-1183): scales the column norms of M (nan_to_num), rotations
+    normalize(matrix_to_quaternion(M / max(scales, 1e-10))), a NaN quaternion -> identity.  `canonical`: C [P,3,3] from
+    complex_canonical_transforms (computed here when None); the result also carries `cell_T`."""
     fl = faces.long()
     V, F = verts.shape[0], fl.shape[0]
     em = torch.ones(F, dtype=torch.bool, device=verts.device) if edition_mask is None else edition_mask.bool()
@@ -394,12 +455,29 @@ def edited_frosting_attributes(params, ref_verts, faces, cells, inner_dist, oute
     inner = verts + vfac[:, None] * inner_dist[:, None] * n
     outer = verts + vfac[:, None] * outer_dist[:, None] * n
     a = frosting_attributes(params, dict(faces=faces, inner=inner, outer=outer, cells=cells))
-    scales = a["scales"].clone()
-    scales[gem] = scales[gem] * gfac
-    q = a["rotations"].clone()
-    fq, rq = face_quaternions(verts, faces), face_quaternions(ref_verts, faces)
     c = cells[gem]
-    q[gem] = quaternion_multiply(fq[c], quaternion_multiply(quaternion_invert(rq[c]), q[gem]))
+    extra = {}
+    if adaptation == "simple":
+        scales = a["scales"].clone()
+        scales[gem] = scales[gem] * gfac
+        q = a["rotations"].clone()
+        fq, rq = face_quaternions(verts, faces), face_quaternions(ref_verts, faces)
+        q[gem] = quaternion_multiply(fq[c], quaternion_multiply(quaternion_invert(rq[c]), q[gem]))
+    elif adaptation == "complex":
+        if canonical is None:
+            canonical, _ = complex_canonical_transforms(params, ref_verts, faces, cells, em, thickness_rescaling)
+        T = cell_transformations(verts, faces, em, thickness_rescaling)
+        M = T[c] @ canonical[gem]
+        s = M.norm(dim=-2)
+        scales = a["scales"].clone()
+        scales[gem] = s
+        scales = scales.nan_to_num()
+        q = a["rotations"].clone()
+        q[gem] = torch.nn.functional.normalize(matrix_to_quaternion(M / s[..., None, :].clamp_min(1e-10)), dim=-1)
+        q[q.isnan().any(dim=-1)] = q.new_tensor([1.0, 0.0, 0.0, 0.0])
+        extra = dict(cell_T=T)
+    else:
+        raise ValueError(f"adaptation {adaptation!r} is not recognized (simple or complex)")
     keep = (cur_d / ref_d).max(dim=-1).values <= deformation_threshold
     opac = a["opacities"].clone()
     opac[gem & ~keep[cells]] = 0.0
@@ -413,7 +491,8 @@ def edited_frosting_attributes(params, ref_verts, faces, cells, inner_dist, oute
         rot = quaternion_to_matrix(quaternion_multiply(q, quaternion_invert(orig_quats)))
         dirs = (dirs[:, None] @ rot)[:, 0]
     colors = sh_colors(shs[:, :(sh_degree + 1) ** 2], dirs, sh_degree)
-    return dict(means3D=pos, opacities=opac, scales=scales, rotations=q, colors_precomp=colors, inner=inner, outer=outer)
+    return dict(means3D=pos, opacities=opac, scales=scales, rotations=q, colors_precomp=colors, inner=inner, outer=outer,
+                **extra)
 
 
 def deform_base(verts, t=1.0, centre=(0.0, 0.0, 6.0)):

@@ -335,6 +335,25 @@ int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_fro
 /* sizeof(fb200_frosting_edit), for binding mirrors */
 size_t fb200_frosting_edit_struct_size(void);
 
+/* Complex adaptation (make_editable(use_simple_adapt=False), frosting_model.py:900-967, :1055-1119, :1149-1183): each
+ * edited Gaussian keeps a canonical transform C = T_ref[cell]^-1 R(q) diag(exp(s)), where T maps a canonical cell to
+ * the world ([a', b', normalize(n) * d]: two Gram-Schmidt-orthogonalised in-plane axes and the normal scaled by the
+ * median distance).  Per frame M = T_frame[cell] C gives the scales (column norms) and the rotation.
+ *
+ * fb200_frosting_edit_complex_capture: run after the reference capture of fb200_frosting_edit_shell (e's d_dists and,
+ * median method, d_factor[0] hold the reference's), with fp the parameter block of that capture.  Writes d_cell_T [F,9]
+ * (row-major 3x3, edited faces only; singular cells fixed up as the reference does), d_canonical [P,9] (0 on unedited
+ * rows) and d_n_singular [1]: the Gaussians whose cell is still singular (their C is 0; the reference's solve fails).
+ * fb200_frosting_edit_attributes_complex: fb200_frosting_edit_attributes with the complex rule for edited rows; run
+ * after this frame's fb200_frosting_edit_shell.  Rewrites d_cell_T for the frame's edited faces. */
+int fb200_frosting_edit_complex_capture(const fb200_frosting_edit* e, const fb200_frosting_params* fp, float* d_cell_T,
+                                        float* d_canonical, uint32_t* d_n_singular, void* stream);
+int fb200_frosting_edit_attributes_complex(const fb200_frosting_edit* e, const fb200_frosting_params* fp,
+                                           int32_t sh_degree, const float* d_campos /*[3]*/, const float* d_orig_quats,
+                                           const float* d_canonical, float* d_cell_T, float* d_means3D,
+                                           float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
+                                           void* stream);
+
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).
  *   d_pred, d_gt [C,H,W]; d_maps [3,C,H,W] scratch kept for backward; d_partials [fb200_loss_partials(C,H,W)];

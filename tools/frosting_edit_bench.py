@@ -1,15 +1,18 @@
 """One frame of an animated Frosting scene: the CUDA edit path against the torch chain a user runs without it.
 
     python tools/frosting_edit_bench.py [--n-bg 0 500000] [--iters 10] [--warmup 3] [--rescaling median]
+                                        [--adaptation simple|complex]
 
 Scene: the C3 frosting layer (2 M mesh-bound Gaussians, ~1 M-face shell, 1920x1080, SH degree 3, ring camera at radius
-6) plus `n_bg` background Gaussians, made editable (simple adaptation, 70 % of the faces edited); every frame bends the
-sphere by a different twist and squash (`scenes.deform_base` at a frame-dependent strength).  Per frame, timed with
+6) plus `n_bg` background Gaussians, made editable (`--adaptation`, simple by default; 70 % of the faces edited); every
+frame bends the sphere by a different twist and squash (`scenes.deform_base` at a frame-dependent strength).  Per frame, timed with
 CUDA events, the two routes alternating:
   (a) `frosting_render_edited` (csrc/frosting_edit.cu: shell + tables, attributes with SH colours; then the rasterizer);
   (b) `scenes.edited_frosting_attributes` -- the torch restatement of the reference's per-frame chain (shell with
-      pytorch3d-style normals, rotations, rescaling, deformation drop, SH colours in torch at rotated directions) --
-      then the same rasterizer with colors_precomp.  The reference's `.median().item()` host read-backs are not in it.
+      pytorch3d-style normals, rotations, rescaling, deformation drop, SH colours in torch at rotated directions; with
+      `--adaptation complex` the cell transforms and T_frame[cell] C, C solved once before the frames as make_editable
+      does) -- then the same rasterizer with colors_precomp.  The reference's `.median().item()` host read-backs are
+      not in it.
 Reports the median of `--iters` frames per route, the max image difference and radii agreement between the routes,
 and the card and its power limit.
 """
@@ -43,13 +46,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--n-mesh", type=int, default=2_000_000)
     ap.add_argument("--rescaling", default="median", choices=["median", "triangle"])
+    ap.add_argument("--adaptation", default="simple", choices=["simple", "complex"])
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     W, H = 1920, 1080
     cam = scenes.ring_cameras(8, W, H, radius=6.0, device=dev)[0]
     rs = scenes.settings_for(cam, 3, device=dev)
     result = {"gpu": torch.cuda.get_device_name(dev), "power_limit": power_limit(), "n_mesh": args.n_mesh,
-              "rescaling": args.rescaling, "runs": []}
+              "rescaling": args.rescaling, "adaptation": args.adaptation, "runs": []}
     e = torch.Tensor([])
     for n_bg in args.n_bg:
         params, mesh = scenes.frosting_layer(args.n_mesh, scenes.make_camera(W, H), 1237,
@@ -61,8 +65,16 @@ def main():
         em = (torch.rand(F, generator=g) < 0.7).to(dev)
         quats = torch.cat([params["quats"], params["bg_quats"]]) if n_bg else params["quats"]
         orig = torch.nn.functional.normalize(quats + 0.2 * torch.randn(quats.shape, generator=g).to(dev), dim=-1)
-        edit = fb.FrostingEdit(mesh["verts"], mesh["faces"], mesh["cells"], inner_dist, outer_dist, edition_mask=em,
-                               thickness_rescaling=args.rescaling)
+        canonical = None
+        if args.adaptation == "simple":
+            edit = fb.FrostingEdit(mesh["verts"], mesh["faces"], mesh["cells"], inner_dist, outer_dist, edition_mask=em,
+                                   thickness_rescaling=args.rescaling)
+        else:
+            edit = fb.FrostingEditComplex(params, mesh["verts"], mesh["faces"], mesh["cells"], inner_dist, outer_dist,
+                                          edition_mask=em, thickness_rescaling=args.rescaling)
+            with torch.no_grad():
+                canonical, _ = scenes.complex_canonical_transforms(params, mesh["verts"], mesh["faces"], mesh["cells"],
+                                                                   em, args.rescaling)
 
         def route_a(verts):
             return fb.frosting_render_edited(params, edit, verts, rs, orig_quats=orig)
@@ -70,7 +82,8 @@ def main():
         def route_b(verts):
             a = scenes.edited_frosting_attributes(params, mesh["verts"], mesh["faces"], mesh["cells"], inner_dist,
                                                   outer_dist, verts, rs.campos, 3, edition_mask=em,
-                                                  thickness_rescaling=args.rescaling, orig_quats=orig)
+                                                  thickness_rescaling=args.rescaling, orig_quats=orig,
+                                                  adaptation=args.adaptation, canonical=canonical)
             color, radii, _, _ = R._launch_forward(a["means3D"], e, a["colors_precomp"], a["opacities"], a["scales"],
                                                    a["rotations"], e, rs, None)
             return color, radii
@@ -103,7 +116,7 @@ def main():
         run["speedup_b_over_a"] = run["b_torch_chain_rasterizer"]["median_ms"] / run["a_frosting_render_edited"]["median_ms"]
         result["runs"].append(run)
         print(json.dumps(run), flush=True)
-        del params, mesh, outs, edit
+        del params, mesh, outs, edit, canonical
         torch.cuda.empty_cache()
     print(json.dumps(result))
 
