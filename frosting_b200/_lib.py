@@ -22,6 +22,7 @@ EXPORTED = [
     "fb200_frosting_attributes", "fb200_frosting_attributes_backward",
     "fb200_frosting_edit_shell", "fb200_frosting_edit_attributes", "fb200_frosting_edit_struct_size",
     "fb200_frosting_edit_complex_capture", "fb200_frosting_edit_attributes_complex",
+    "fb200_frosting_skin_pose", "fb200_frosting_skin_struct_size",
     "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
@@ -101,6 +102,12 @@ class FrostingEdit(C.Structure):
                                           "d_ref_dists", "d_ref_median", "d_dists", "d_face_normals", "d_rel_quats",
                                           "d_face_factor", "d_face_keep", "d_factor", "d_select", "d_inner_verts",
                                           "d_outer_verts")]
+
+
+class FrostingSkin(C.Structure):
+    _fields_ = [("n_rows", C.c_int32), ("n_verts", C.c_int32), ("n_bones", C.c_int32), ("n_frames", C.c_int32)] + \
+               [(n, C.c_void_p) for n in ("d_tpose", "d_vert_ids", "d_offsets", "d_bones", "d_weights", "d_reset",
+                                          "d_pose")]
 
 
 ADAM_MAX_GROUPS = 16
@@ -187,6 +194,9 @@ def lib():
     L.fb200_frosting_edit_attributes_complex.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams),
                                                          C.c_int32] + [C.c_void_p] * 10
     L.fb200_frosting_edit_attributes_complex.restype = C.c_int
+    L.fb200_frosting_skin_pose.argtypes = [C.POINTER(FrostingSkin), C.c_int32, C.c_void_p, C.c_void_p]
+    L.fb200_frosting_skin_pose.restype = C.c_int
+    L.fb200_frosting_skin_struct_size.restype = C.c_size_t
     L.fb200_loss_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.fb200_loss_partials.restype = C.c_size_t
     L.fb200_l1_dssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
@@ -223,6 +233,8 @@ def lib():
                            f"{[int(x) for x in sizes]} vs {[C.sizeof(m) for m in mirrors]}")
     if L.fb200_frosting_edit_struct_size() != C.sizeof(FrostingEdit):
         raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_edit out of sync with include/frosting_b200.h")
+    if L.fb200_frosting_skin_struct_size() != C.sizeof(FrostingSkin):
+        raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_skin out of sync with include/frosting_b200.h")
     _lib = L
     return L
 

@@ -598,6 +598,25 @@ int fb200_frosting_edit_attributes_complex(const fb200_frosting_edit* e, const f
                  "frosting_edit_attributes_complex");
 }
 
+size_t fb200_frosting_skin_struct_size(void) { return sizeof(fb200_frosting_skin); }
+
+int fb200_frosting_skin_pose(const fb200_frosting_skin* s, int32_t frame, float* d_base_verts, void* stream) {
+    if (!s) return fail(FB200_EINVAL, "frosting_skin: null skin struct%s");
+    if (s->n_rows < 0 || s->n_verts < 0 || s->n_bones < 0 || s->n_frames < 0 || s->n_rows > s->n_verts)
+        return fail(FB200_EINVAL, "frosting_skin: bad extents%s");
+    if (frame < 0 || frame >= s->n_frames)
+        return fail(FB200_EINVAL, "frosting_skin: frame outside [0, n_frames)%s");
+    if (s->n_rows > 0 && (!s->d_tpose || !s->d_vert_ids || !s->d_offsets || !d_base_verts))
+        return fail(FB200_EINVAL, "frosting_skin: missing vertex table pointer%s");
+    if (s->n_rows > 0 && s->n_bones > 0 && (!s->d_bones || !s->d_weights || !s->d_reset || !s->d_pose))
+        return fail(FB200_EINVAL, "frosting_skin: missing bone table pointer%s");
+    if ((reinterpret_cast<uintptr_t>(s->d_reset) & 15) || (reinterpret_cast<uintptr_t>(s->d_pose) & 15))
+        return fail(FB200_EINVAL, "frosting_skin: reset / pose matrices must be 16-byte aligned%s");
+    if (s->n_rows == 0) return FB200_OK;
+    return check(launch_frosting_skin(*s, frame, d_base_verts, static_cast<cudaStream_t>(stream)),
+                 "frosting_skin_pose");
+}
+
 size_t fb200_loss_partials(int32_t C, int32_t H, int32_t W) {
     return (C > 0 && H > 0 && W > 0) ? l1_dssim_num_partials(C, H, W) : 0;
 }

@@ -508,3 +508,131 @@ def deform_base(verts, t=1.0, centre=(0.0, 0.0, 6.0)):
     x = x * (1.0 + 0.35 * t) + 0.08 * t * p[:, 1] ** 2
     z = z * (1.0 - 0.25 * t)
     return torch.stack([x, y, z], -1) + c
+
+
+# ---- Blender-animated scenes: apply_poses_to_scene (blender/frosting_utils.py:474-516), restated ----
+# pytorch3d's Transform3d is restated from its documented maths (a [N,4,4] matrix in the row-vector convention; inverse
+# by torch.inverse; transform_points = [p, 1] @ M, then the divide by the homogeneous coordinate); the golden generator
+# (tests/golden/make_frosting_skin_golden.py) runs the reference's own source on top of it.
+
+class Transform3d:
+    """The slice of pytorch3d.transforms.Transform3d the reference's skinning uses."""
+
+    def __init__(self, dtype=torch.float32, device="cpu", matrix=None):
+        self._matrix = torch.eye(4, dtype=dtype, device=device).view(1, 4, 4) if matrix is None else matrix.view(-1, 4, 4)
+
+    def get_matrix(self):
+        return self._matrix.clone()
+
+    def inverse(self):
+        return Transform3d(matrix=torch.inverse(self._matrix))
+
+    def transform_points(self, points):
+        pts = points.clone()
+        if pts.dim() == 2:
+            pts = pts[None]
+        N, P, _ = pts.shape
+        pts = torch.cat([pts, torch.ones(N, P, 1, dtype=points.dtype, device=points.device)], dim=2)
+        m = self.get_matrix()
+        if m.shape[0] != N:
+            m = m.expand(N, -1, -1)
+        out = pts.bmm(m)
+        out = out[..., :3] / out[..., 3:]
+        if out.shape[0] == 1 and points.dim() == 2:
+            out = out.reshape(points.shape)
+        return out
+
+
+def skin_vertices(package, ref_indices, i_frame, base_verts):
+    """apply_poses_to_scene's loop in torch: writes frame `i_frame` (wrapped by the package's frame count) of every rigged
+    mesh's range [ref_indices[i], ref_indices[i+1]) of `base_verts` in place and returns it.  `package`: as
+    load_blender_package leaves it (float64 weights in `bone_to_vertex_weights`).  The oracle of frosting_b200.skin."""
+    n_frames = len(package["camera"]["lens"])
+    with torch.no_grad():
+        for i_mesh, mesh_dict in enumerate(package["bones"]):
+            if not mesh_dict:
+                continue
+            idx_of, w_of = package["bone_to_vertices"][i_mesh], package["bone_to_vertex_weights"][i_mesh]
+            tpose, arm = mesh_dict["vertex"]["tpose_points"], mesh_dict["armature"]
+            new_points = torch.zeros_like(tpose)
+            for bone, idx in idx_of.items():
+                if len(idx) > 0:
+                    pose_t = Transform3d(matrix=arm["pose_bones"][bone][i_frame % n_frames].transpose(-1, -2))
+                    reset_t = Transform3d(matrix=arm["rest_bones"][bone].transpose(-1, -2)).inverse()
+                    new_points[idx] += w_of[bone][..., None] * pose_t.transform_points(
+                        reset_t.transform_points(tpose[idx]))
+            base_verts[ref_indices[i_mesh]:ref_indices[i_mesh + 1]] = new_points
+    return base_verts
+
+
+def _translation(t):
+    m = torch.eye(4, dtype=torch.float64)
+    m[:3, 3] = t
+    return m
+
+
+def _rotation(axis, a):
+    c, s = math.cos(a), math.sin(a)
+    i, j = [(1, 2), (2, 0), (0, 1)][axis]
+    m = torch.eye(4, dtype=torch.float64)
+    m[i, i], m[i, j], m[j, i], m[j, j] = c, -s, s, c
+    return m
+
+
+def skinned_rig(verts, n_bones, n_frames, seed=0):
+    """A rig over the whole of `verts` (one mesh) as load_blender_package leaves a Blender package -- the keys
+    apply_poses_to_scene reads -- and its ref_indices [0, V].  The tracks are the animation's frames.
+
+    The rig is a chain of `n_bones` bones up the y extent of the mesh, T-pose = `verts`.  A vertex at chain coordinate
+    u (in bone lengths) takes every bone whose centre lies within h of u, with weight 1 - |u - centre| / h normalised in
+    float64; h runs from 0.6 to 2 around the chain, so a vertex has one bone near a bone's centre and up to four in the
+    blend zones.  Frame f bends each bone about z and x by angles that vary with the frame and the bone (at most
+    0.6 / n_bones and 0.3 / n_bones rad per bone), and moves the root."""
+    dev = verts.device
+    v = verts.detach().cpu().double()
+    lo, hi = v.min(0).values, v.max(0).values
+    c = (lo + hi) / 2
+    L = float(hi[1] - lo[1]) / n_bones
+    u = ((v[:, 1] - lo[1]) / L).clamp(0.0, n_bones - 1e-6)
+    h = 0.6 + 0.7 * (1.0 + torch.sin(3.0 * torch.atan2(v[:, 2] - c[2], v[:, 0] - c[0])))
+    rows, bones, ws = [], [], []
+    for j in range(-2, 3):
+        k = u.floor().long() + j
+        w = (1.0 - (u - (k.double() + 0.5)).abs() / h).clamp_min(0.0)
+        ok = (k >= 0) & (k < n_bones) & (w > 0)
+        rows.append(torch.nonzero(ok)[:, 0])
+        bones.append(k[ok])
+        ws.append(w[ok])
+    rows, bones, ws = torch.cat(rows), torch.cat(bones), torch.cat(ws)
+    ws = ws / torch.zeros(v.shape[0], dtype=torch.float64).index_add(0, rows, ws)[rows]
+    order = torch.argsort(bones * v.shape[0] + rows)
+    rows, bones, ws = rows[order], bones[order], ws[order]
+    counts = torch.bincount(bones, minlength=n_bones).tolist()
+    names = [f"bone_{k:03d}" for k in range(n_bones)]
+    heads = [torch.tensor([float(c[0]), float(lo[1]) + k * L, float(c[2])], dtype=torch.float64) for k in range(n_bones)]
+    g = torch.Generator().manual_seed(seed)
+    phase = torch.rand(n_bones, 2, generator=g, dtype=torch.float64) * 2 * math.pi
+    rest, pose = {}, {}
+    tracks = torch.empty(n_bones, n_frames, 4, 4, dtype=torch.float64)
+    for f in range(n_frames):
+        t = 2 * math.pi * f / n_frames
+        parent = _translation(heads[0] + torch.tensor([0.1 * math.sin(t), 0.0, 0.05 * math.cos(t)], dtype=torch.float64))
+        for k in range(n_bones):
+            if k > 0:
+                parent = tracks[k - 1, f] @ _translation(heads[k] - heads[k - 1])
+            rot = _rotation(2, 0.6 / n_bones * math.sin(t + phase[k, 0].item())) @ \
+                _rotation(0, 0.3 / n_bones * math.cos(t + phase[k, 1].item()))
+            tracks[k, f] = parent @ rot
+    for k, name in enumerate(names):
+        rest[name] = _translation(heads[k]).float().to(dev)
+        pose[name] = tracks[k].float().to(dev)
+    idx_of, w_of = {}, {}
+    for name, chunk_r, chunk_w in zip(names, rows.split(counts), ws.split(counts)):
+        idx_of[name] = chunk_r.to(dev) if len(chunk_r) else []
+        w_of[name] = chunk_w.to(dev) if len(chunk_w) else []
+    eye = torch.eye(4, device=dev)
+    package = {"camera": {"lens": torch.full((n_frames,), 50.0)},
+               "bones": [{"vertex": {"tpose_points": verts.detach().float().contiguous(), "matrix_world": eye},
+                          "armature": {"matrix_world": eye, "rest_bones": rest, "pose_bones": pose}}],
+               "bone_to_vertices": [idx_of], "bone_to_vertex_weights": [w_of]}
+    return package, [0, v.shape[0]]

@@ -354,6 +354,32 @@ int fb200_frosting_edit_attributes_complex(const fb200_frosting_edit* e, const f
                                            float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
                                            void* stream);
 
+/* Linear-blend skinning of a Blender-animated scene's base mesh (blender/frosting_utils.py:474-516
+ * apply_poses_to_scene).  Row i of the rigged vertices is base vertex d_vert_ids[i]; its entries
+ * [d_offsets[i], d_offsets[i+1]) are (bone, weight) pairs in the armature's bone order.  Per entry:
+ *   q = [p, 1] @ d_reset[bone], q = q.xyz / q.w;  r = [q, 1] @ d_pose[bone][frame], r = r.xyz / r.w;
+ *   acc = (float)((double)acc + weight * (double)r)
+ * starting from acc = 0; the vertex is set to acc (0 without entries).  Base vertices that are no row's are neither
+ * read nor written.  Matrices are row-major 4x4 in the row-vector convention (pytorch3d's Transform3d):
+ * d_reset = inverse(rest^T), d_pose = the track's matrices transposed; both 16-byte aligned. */
+typedef struct fb200_frosting_skin {
+    int32_t n_rows;                 /* rigged vertices */
+    int32_t n_verts;                /* rows of the base-vertex buffer (d_vert_ids < n_verts) */
+    int32_t n_bones;
+    int32_t n_frames;               /* frames of every pose track */
+    const float* d_tpose;           /* [n_rows,3] T-pose points */
+    const int32_t* d_vert_ids;      /* [n_rows] */
+    const int32_t* d_offsets;       /* [n_rows+1] CSR into d_bones / d_weights */
+    const int32_t* d_bones;         /* [n_entries] bone ids in [0, n_bones) */
+    const double* d_weights;        /* [n_entries] normalised weights (float64, as the reference keeps them) */
+    const float* d_reset;           /* [n_bones,4,4] */
+    const float* d_pose;            /* [n_bones,n_frames,4,4] */
+} fb200_frosting_skin;
+/* Writes frame `frame` (in [0, n_frames)) into d_base_verts [n_verts,3] in place.  One launch, no allocation. */
+int fb200_frosting_skin_pose(const fb200_frosting_skin* s, int32_t frame, float* d_base_verts, void* stream);
+/* sizeof(fb200_frosting_skin), for binding mirrors */
+size_t fb200_frosting_skin_struct_size(void);
+
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).
  *   d_pred, d_gt [C,H,W]; d_maps [3,C,H,W] scratch kept for backward; d_partials [fb200_loss_partials(C,H,W)];
