@@ -23,6 +23,8 @@ EXPORTED = [
     "fb200_frosting_edit_shell", "fb200_frosting_edit_attributes", "fb200_frosting_edit_struct_size",
     "fb200_frosting_edit_complex_capture", "fb200_frosting_edit_attributes_complex",
     "fb200_frosting_skin_pose", "fb200_frosting_skin_struct_size",
+    "fb200_mesh_barycentrics", "fb200_texture_face_sh_colours", "fb200_texture_add_view", "fb200_texture_finish",
+    "fb200_texture_struct_size",
     "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
@@ -108,6 +110,12 @@ class FrostingSkin(C.Structure):
     _fields_ = [("n_rows", C.c_int32), ("n_verts", C.c_int32), ("n_bones", C.c_int32), ("n_frames", C.c_int32)] + \
                [(n, C.c_void_p) for n in ("d_tpose", "d_vert_ids", "d_offsets", "d_bones", "d_weights", "d_reset",
                                           "d_pose")]
+
+
+class Texture(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_faces", "n_points", "square_size", "n_square_per_axis", "texture_size")] + \
+               [(n, C.c_void_p) for n in ("d_cell_offsets", "d_cell_points", "d_sh_dc", "d_face_sh", "d_face_acc",
+                                          "d_texel_acc", "d_face_winner", "d_texel_winner")]
 
 
 ADAM_MAX_GROUPS = 16
@@ -197,6 +205,16 @@ def lib():
     L.fb200_frosting_skin_pose.argtypes = [C.POINTER(FrostingSkin), C.c_int32, C.c_void_p, C.c_void_p]
     L.fb200_frosting_skin_pose.restype = C.c_int
     L.fb200_frosting_skin_struct_size.restype = C.c_size_t
+    L.fb200_mesh_barycentrics.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                          C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.fb200_texture_face_sh_colours.argtypes = [C.POINTER(Texture), C.c_void_p]
+    L.fb200_texture_add_view.argtypes = [C.POINTER(Texture), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_void_p]
+    L.fb200_texture_finish.argtypes = [C.POINTER(Texture), C.c_void_p, C.c_void_p]
+    for n in ("fb200_mesh_barycentrics", "fb200_texture_face_sh_colours", "fb200_texture_add_view",
+              "fb200_texture_finish"):
+        getattr(L, n).restype = C.c_int
+    L.fb200_texture_struct_size.restype = C.c_size_t
     L.fb200_loss_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     L.fb200_loss_partials.restype = C.c_size_t
     L.fb200_l1_dssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
@@ -235,6 +253,8 @@ def lib():
         raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_edit out of sync with include/frosting_b200.h")
     if L.fb200_frosting_skin_struct_size() != C.sizeof(FrostingSkin):
         raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_skin out of sync with include/frosting_b200.h")
+    if L.fb200_texture_struct_size() != C.sizeof(Texture):
+        raise RuntimeError("frosting_b200: ctypes mirror of fb200_texture out of sync with include/frosting_b200.h")
     _lib = L
     return L
 

@@ -617,6 +617,61 @@ int fb200_frosting_skin_pose(const fb200_frosting_skin* s, int32_t frame, float*
                  "frosting_skin_pose");
 }
 
+int fb200_mesh_barycentrics(int32_t V, int32_t F, const float* d_verts, const int32_t* d_faces,
+                            const float* d_full_proj, int32_t W, int32_t H, const int32_t* d_pix_to_face,
+                            float* d_bary, void* stream) {
+    if (V < 0 || F < 0 || W <= 0 || H <= 0 || (int64_t)W * H > INT32_MAX || !d_full_proj || !d_pix_to_face ||
+        !d_bary || (F > 0 && (!d_verts || !d_faces)))
+        return fail(FB200_EINVAL, "mesh_barycentrics: bad arguments%s");
+    return check(launch_mesh_bary(F, d_verts, d_faces, d_full_proj, W, H, d_pix_to_face, d_bary,
+                                  static_cast<cudaStream_t>(stream)),
+                 "mesh_barycentrics");
+}
+
+size_t fb200_texture_struct_size(void) { return sizeof(fb200_texture); }
+
+namespace {
+
+int check_texture(const fb200_texture* t) {
+    if (!t) return fail(FB200_EINVAL, "texture: null texture struct%s");
+    const int64_t n = t->n_square_per_axis;
+    if (t->n_faces < 1 || t->n_points < 0 || t->square_size < 3 || n < 1 || 2 * n * n < t->n_faces ||
+        (int64_t)t->square_size * n != t->texture_size || (int64_t)t->texture_size * t->texture_size > INT32_MAX)
+        return fail(FB200_EINVAL, "texture: bad extents (F >= 1, square_size >= 3, 2 n^2 >= F, T = square_size n)%s");
+    if (!t->d_cell_offsets || (t->n_points > 0 && (!t->d_cell_points || !t->d_sh_dc)) || !t->d_face_sh)
+        return fail(FB200_EINVAL, "texture: missing face table pointer%s");
+    if (!t->d_face_acc || !t->d_texel_acc || !t->d_face_winner || !t->d_texel_winner)
+        return fail(FB200_EINVAL, "texture: missing accumulator / winner pointer%s");
+    if ((reinterpret_cast<uintptr_t>(t->d_face_acc) & 15) || (reinterpret_cast<uintptr_t>(t->d_texel_acc) & 15))
+        return fail(FB200_EINVAL, "texture: accumulators must be 16-byte aligned%s");
+    return FB200_OK;
+}
+
+}  // namespace
+
+int fb200_texture_face_sh_colours(const fb200_texture* t, void* stream) {
+    int rc = check_texture(t);
+    if (rc != FB200_OK) return rc;
+    return check(launch_texture_face_sh(*t, static_cast<cudaStream_t>(stream)), "texture_face_sh_colours");
+}
+
+int fb200_texture_add_view(const fb200_texture* t, const float* d_image, const int32_t* d_pix_to_face,
+                           const float* d_bary, int32_t W, int32_t H, void* stream) {
+    int rc = check_texture(t);
+    if (rc != FB200_OK) return rc;
+    if (W <= 0 || H <= 0 || (int64_t)W * H > INT32_MAX || !d_image || !d_pix_to_face || !d_bary)
+        return fail(FB200_EINVAL, "texture_add_view: bad arguments%s");
+    return check(launch_texture_add_view(*t, d_image, d_pix_to_face, d_bary, W * H, static_cast<cudaStream_t>(stream)),
+                 "texture_add_view");
+}
+
+int fb200_texture_finish(const fb200_texture* t, float* d_texture, void* stream) {
+    int rc = check_texture(t);
+    if (rc != FB200_OK) return rc;
+    if (!d_texture) return fail(FB200_EINVAL, "texture_finish: missing output%s");
+    return check(launch_texture_fill(*t, d_texture, static_cast<cudaStream_t>(stream)), "texture_finish");
+}
+
 size_t fb200_loss_partials(int32_t C, int32_t H, int32_t W) {
     return (C > 0 && H > 0 && W > 0) ? l1_dssim_num_partials(C, H, W) : 0;
 }

@@ -636,3 +636,90 @@ def skinned_rig(verts, n_bones, n_frames, seed=0):
                           "armature": {"matrix_world": eye, "rest_bones": rest, "pose_bones": pose}}],
                "bone_to_vertices": [idx_of], "bone_to_vertex_weights": [w_of]}
     return package, [0, v.shape[0]]
+
+
+# ---- texture bake (SURVEY.md row a22): compute_textured_mesh_for_frosting_mesh, restated ----
+SH_C0 = 0.28209479177387814          # frosting_utils/spherical_harmonics.py C0; SH2RGB(sh) = sh * C0 + 0.5
+
+
+def texture_uv_layout(n_faces, square_size, device="cpu"):
+    """The UV atlas of texture.py:30-71: (verts_uv [6 n^2, 2] float32, faces_uv [F,3] int64, n, T).  Face f uses UV
+    vertices 3f..3f+2 -- half f % 2 of square f // 2, whose cell (i, j) = divmod(f // 2, n) -- with inset corners.
+    The division by T is IEEE fp32 on either device, as in the reference run on the CPU and in csrc/texture.cu: T is a
+    tensor on `device` (torch's CUDA division by a Python scalar multiplies by its reciprocal instead)."""
+    n = int(math.sqrt(n_faces // 2 + 1) + 1)
+    T = square_size * n
+    ij = torch.cartesian_prod(torch.arange(n, device=device), torch.arange(n, device=device))[:, None]
+    u = torch.tensor([[1, 0]], dtype=torch.int32, device=device)[:, None]
+    v = torch.tensor([[0, 1]], dtype=torch.int32, device=device)[:, None]
+    uv = torch.cat([ij + u, ij, ij + u + v, ij + v, ij, ij + u + v], dim=1) * square_size
+    uv = uv + torch.tensor([[-2, 1], [2, 1], [-2, -3], [1, -1], [1, 3], [-3, -1]], device=device)
+    verts_uv = uv.reshape(-1, 2).float() / torch.tensor(float(T), device=device)
+    faces_uv = torch.arange(3 * n_faces, device=device).view(n_faces, 3)
+    return verts_uv, faces_uv, n, T
+
+
+def _last_wins(idx, n):
+    """Positions (into idx) of the last occurrence of every distinct value: the entries that
+    `acc[idx] = acc[idx] + x` keeps when idx has duplicates and runs in order, as it does on the CPU."""
+    pos = torch.arange(idx.shape[0], device=idx.device)
+    win = torch.full((n,), -1, dtype=torch.long, device=idx.device).scatter_reduce_(0, idx, pos, "amax")
+    return win[win >= 0]
+
+
+def bake_texture_torch(n_faces, cells, sh_dc, square_size, images, pix_to_faces, barys):
+    """texture.py:11-166 in torch over given views: images [H,W,3] (the render, before nan_to_num / clamp),
+    pix_to_faces [H,W] (-1: background) and barys [H,W,3].  Returns (verts_uv, faces_uv, texture [T,T,3]).
+
+    The per-view `acc[idx] = acc[idx] + colors` keeps the last pixel in row-major order of every face and texel
+    (_last_wins), as the reference does on the CPU, so the bake is deterministic on either device.  The reference's count
+    clamp of the SH colours is an expression whose result is dropped: a face with neither Gaussians nor hits is 0 / 0 =
+    NaN, kept here.  Works on CPU and CUDA tensors alike (the CPU run is the oracle of frosting_b200.texture)."""
+    device = cells.device
+    F = int(n_faces)
+    verts_uv, faces_uv, n, T = texture_uv_layout(F, square_size, device)
+    uvs = torch.cartesian_prod(torch.arange(T, device=device, dtype=torch.int32),
+                               torch.arange(T, device=device, dtype=torch.int32)).view(T, T, 2)
+    square = uvs // square_size
+    square = square[..., 0] * n + square[..., 1]
+    in_top = uvs % square_size
+    in_top = in_top[..., 0] < in_top[..., 1]
+    uv_to_faces = (2 * square + in_top).transpose(0, 1).clamp_max(F - 1)
+    del uvs, square, in_top
+
+    texture_img = torch.zeros(T, T, 3, device=device)
+    texture_count = torch.zeros(T, T, 1, device=device)
+    face_colors = torch.zeros(F, 3, device=device)
+    face_count = torch.zeros(F, 1, device=device)
+    cells = cells.long()
+    sh_colors = torch.zeros_like(face_colors).index_add_(0, cells, (sh_dc.reshape(-1, 3) * SH_C0 + 0.5).clamp(0., 1.))
+    sh_counts = torch.zeros_like(face_count).index_add_(0, cells, torch.ones_like(cells[..., None]).float())
+    sh_colors = sh_colors / sh_counts
+
+    for image, p2f, bary in zip(images, pix_to_faces, barys):
+        rgb = image.nan_to_num().clamp(min=0, max=1).reshape(-1, 3)
+        p2f = p2f.reshape(-1).long()
+        mask = p2f > -1
+        face_indices, colors = p2f[mask], rgb[mask]
+        bary = bary.reshape(-1, 3)[mask]
+        w = _last_wins(face_indices, F)
+        fw = face_indices[w]
+        face_count[fw] = face_count[fw] + 1
+        face_colors[fw] = face_colors[fw] + colors[w]
+        pix = ((verts_uv[faces_uv[face_indices]] * bary[:, :, None]).sum(dim=1) * T).int()
+        ok = ((pix >= 0) & (pix < T)).all(dim=1)
+        t = pix[:, 1].long() * T + pix[:, 0].long()
+        t = torch.where(ok, t, T * T)                  # outside the texture: a slot past the end, dropped
+        w = _last_wins(t, T * T + 1)
+        w = w[t[w] < T * T]
+        row, col = pix[w, 1].long(), pix[w, 0].long()
+        texture_img[row, col] = texture_img[row, col] + colors[w]
+        texture_count[row, col] = texture_count[row, col] + 1
+
+    filled = texture_count[..., 0] > 0
+    texture_img[filled] = texture_img[filled] / texture_count[filled]
+    visited = face_count[..., 0] > 0
+    face_colors[visited] = face_colors[visited] / face_count[visited]
+    face_colors[~visited] = sh_colors[~visited]
+    texture_img[~filled] = face_colors[uv_to_faces[~filled]]
+    return verts_uv, faces_uv, texture_img.flip(0)

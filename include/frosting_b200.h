@@ -380,6 +380,45 @@ int fb200_frosting_skin_pose(const fb200_frosting_skin* s, int32_t frame, float*
 /* sizeof(fb200_frosting_skin), for binding mirrors */
 size_t fb200_frosting_skin_struct_size(void);
 
+/* Texture bake of the base mesh (frosting_utils/texture.py:11-181 compute_textured_mesh_for_frosting_mesh).
+ *
+ * fb200_mesh_barycentrics: perspective-correct barycentrics d_bary [H,W,3] of the faces d_pix_to_face [H,W] (from
+ * fb200_mesh_visibility with the same vertices, faces and d_full_proj [4,4]); (u, v, 1 - (u + v)) on a hit,
+ * (0, 0, 1) elsewhere.
+ *
+ * Face f owns half f % 2 of UV square f / 2 (square s at texels [s / n * sq, +sq) x [s % n * sq, +sq)).  Per view,
+ * every touched face and texel receives ONE pixel's colour and a count of 1: the last hit pixel in row-major order
+ * (what `acc[idx] = acc[idx] + colors` with duplicate indices does on the CPU).  Accumulation is fp32 in view order.
+ * The caller zeroes d_face_acc / d_texel_acc and sets d_face_winner / d_texel_winner to -1 once; every view leaves the
+ * winner slots at -1 again.  A face without Gaussians and without a view hit gets NaN, as in the reference. */
+typedef struct fb200_texture {
+    int32_t n_faces;                /* F >= 1 */
+    int32_t n_points;               /* mesh-bound Gaussians */
+    int32_t square_size;            /* sq >= 3 */
+    int32_t n_square_per_axis;      /* n, with 2 n^2 >= F */
+    int32_t texture_size;           /* T = sq * n */
+    const int32_t* d_cell_offsets;  /* [F+1] CSR face -> Gaussians */
+    const int32_t* d_cell_points;   /* [n_points] Gaussian ids, ascending within each face */
+    const float* d_sh_dc;           /* [n_points,3] SH degree-0 coefficients */
+    float* d_face_sh;               /* [F,3] written by fb200_texture_face_sh_colours */
+    float* d_face_acc;              /* [F,4] colour sum and count, 16-byte aligned */
+    float* d_texel_acc;             /* [T*T,4] colour sum and count per texel (row-major, before the flip) */
+    int32_t* d_face_winner;         /* [F] */
+    int32_t* d_texel_winner;        /* [T*T] */
+} fb200_texture;
+int fb200_mesh_barycentrics(int32_t V, int32_t F, const float* d_verts, const int32_t* d_faces,
+                            const float* d_full_proj, int32_t W, int32_t H, const int32_t* d_pix_to_face,
+                            float* d_bary, void* stream);
+/* Once per bake, before fb200_texture_finish: mean of clamp(SH2RGB(dc), 0, 1) per face into d_face_sh. */
+int fb200_texture_face_sh_colours(const fb200_texture* t, void* stream);
+/* One view: d_image [H,W,3] (nan_to_num and clamp(0, 1) are applied here), d_pix_to_face [H,W], d_bary [H,W,3]. */
+int fb200_texture_add_view(const fb200_texture* t, const float* d_image, const int32_t* d_pix_to_face,
+                           const float* d_bary, int32_t W, int32_t H, void* stream);
+/* d_texture [T,T,3]: filled texels sum / count, others their face's colour; rows flipped (row 0 is v = T-1). */
+int fb200_texture_finish(const fb200_texture* t, float* d_texture, void* stream);
+/* sizeof(fb200_texture), for binding mirrors */
+size_t fb200_texture_struct_size(void);
+
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).
  *   d_pred, d_gt [C,H,W]; d_maps [3,C,H,W] scratch kept for backward; d_partials [fb200_loss_partials(C,H,W)];
