@@ -6,8 +6,7 @@ by hand-written CUDA behind the C ABI of include/frosting_b200.h.  See DESIGN.md
 """
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, rasterize_gaussians,
                          forward_with_state)
-from .frosting_attrs import frosting_attributes_fused
-from .frosting_render import frosting_render, frosting_render_two_step
+from .frosting_render import frosting_attributes_fused, frosting_render, frosting_render_two_step
 from .edit import FrostingEdit, FrostingEditComplex, frosting_render_edited
 from .skin import FrostingSkin, skin_tables
 from .texture import TextureBaker, compute_textured_mesh, mesh_bary, write_textured_obj

@@ -6,6 +6,8 @@ and every op in this package fails loudly.  PyTorch is used only for device memo
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfrosting_b200.so")
 
@@ -272,6 +274,16 @@ def profile_read():
 
 def kernel_launches() -> int:
     return int(lib().fb200_kernel_launches())
+
+
+def ptr(t):
+    """A tensor's device pointer as a `d_*` argument: NULL for a missing or empty tensor."""
+    return None if t is None or t.numel() == 0 else C.c_void_p(t.data_ptr())
+
+
+def stream(device):
+    """The current CUDA stream of `device` as the `void* stream` argument."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 class Fb200Error(RuntimeError):

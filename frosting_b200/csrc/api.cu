@@ -36,6 +36,11 @@ int stage(cudaError_t e, const char* what, bool debug, cudaStream_t s) {
     return FB200_OK;
 }
 
+bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+
+// fb200_frosting_params, for every entry point that reads it.  The alignment is what the kernels' vector accesses need
+// (header: fb200_frosting_params): bary logits as float2, quats as float4, and the sh_rest rows moved as float4 blocks of
+// a warp's 32 rows (frosting_attr.cu)
 int check_frosting(const fb200_frosting_params* fp) {
     if (!fp) return fail(FB200_EINVAL, "frosting_attributes: null params%s");
     if (fp->P < 0 || fp->sh_rest < 0 || fp->n_verts < 0 || fp->n_faces < 0)
@@ -44,20 +49,32 @@ int check_frosting(const fb200_frosting_params* fp) {
                       !fp->d_opacity_logits || !fp->d_log_scales || !fp->d_quats || !fp->d_sh_dc ||
                       (fp->sh_rest > 0 && !fp->d_sh_rest)))
         return fail(FB200_EINVAL, "frosting_attributes: missing parameter pointer%s");
-    if (fp->P > 0 && ((reinterpret_cast<uintptr_t>(fp->d_bary_logits) & 7) || (reinterpret_cast<uintptr_t>(fp->d_quats) & 15)))
-        return fail(FB200_EINVAL, "frosting_attributes: bary logits must be 8-byte, quats 16-byte aligned%s");
+    if (fp->P > 0 && (misaligned(fp->d_bary_logits, 8) || misaligned(fp->d_quats, 16) ||
+                      (fp->sh_rest > 0 && misaligned(fp->d_sh_rest, 16))))
+        return fail(FB200_EINVAL, "frosting_attributes: bary logits must be 8-byte, quats and sh_rest 16-byte aligned%s");
     // background Gaussians
     if (fp->n_bg < 0) return fail(FB200_EINVAL, "frosting background: n_bg must be >= 0%s");
     if (fp->n_bg > 0 && (!fp->d_bg_points || !fp->d_bg_opacity_logits || !fp->d_bg_log_scales || !fp->d_bg_quats ||
                          !fp->d_bg_sh_dc || (fp->sh_rest > 0 && !fp->d_bg_sh_rest)))
         return fail(FB200_EINVAL, "frosting background: missing parameter pointer%s");
-    if (fp->n_bg > 0 && (reinterpret_cast<uintptr_t>(fp->d_bg_quats) & 15))
+    if (fp->n_bg > 0 && misaligned(fp->d_bg_quats, 16))
         return fail(FB200_EINVAL, "frosting background: quats must be 16-byte aligned%s");
     return FB200_OK;
 }
 
-// the background rows of a parameter-gradient block: given exactly when there are background Gaussians
-int check_background_grads(const fb200_frosting_params* fp, const fb200_frosting_grads* g) {
+// fb200_frosting_grads over the block fp, for fb200_backward (frosting mode) and fb200_frosting_attributes_backward.
+// Mesh rows (fp->P > 0): every parameter gradient, the shell's both or neither, each base 16-byte aligned (the
+// attribute backward zero-fills a warp's rows with float4 stores and stores quats as float4).  Background rows: given
+// exactly when there are background Gaussians, quats stored as float4.
+int check_frosting_grads(const fb200_frosting_params* fp, const fb200_frosting_grads* g) {
+    if (!g) return fail(FB200_EINVAL, "frosting gradients: null gradient block%s");
+    if (fp->P > 0 && (!g->d_bary_logits || !g->d_opacity_logits || !g->d_log_scales || !g->d_quats || !g->d_sh_dc ||
+                      (fp->sh_rest > 0 && !g->d_sh_rest) || ((g->d_inner_verts == nullptr) != (g->d_outer_verts == nullptr))))
+        return fail(FB200_EINVAL, "frosting gradients: parameter-gradient pointers missing%s");
+    if (fp->P > 0 && (misaligned(g->d_bary_logits, 16) || misaligned(g->d_opacity_logits, 16) ||
+                      misaligned(g->d_log_scales, 16) || misaligned(g->d_quats, 16) || misaligned(g->d_sh_dc, 16) ||
+                      (fp->sh_rest > 0 && misaligned(g->d_sh_rest, 16))))
+        return fail(FB200_EINVAL, "frosting gradients: the mesh parameter gradients must be 16-byte aligned%s");
     const bool any = g->d_bg_points || g->d_bg_opacity_logits || g->d_bg_log_scales || g->d_bg_quats || g->d_bg_sh_dc ||
                      g->d_bg_sh_rest;
     if (any != (fp->n_bg > 0))
@@ -66,7 +83,7 @@ int check_background_grads(const fb200_frosting_params* fp, const fb200_frosting
     if (fp->n_bg > 0 && (!g->d_bg_points || !g->d_bg_opacity_logits || !g->d_bg_log_scales || !g->d_bg_quats ||
                          !g->d_bg_sh_dc || (fp->sh_rest > 0 && !g->d_bg_sh_rest)))
         return fail(FB200_EINVAL, "frosting background: gradient pointers missing%s");
-    if (fp->n_bg > 0 && (reinterpret_cast<uintptr_t>(g->d_bg_quats) & 15))
+    if (fp->n_bg > 0 && misaligned(g->d_bg_quats, 16))
         return fail(FB200_EINVAL, "frosting background: dL/dquats must be 16-byte aligned%s");
     return FB200_OK;
 }
@@ -84,8 +101,6 @@ int validate_frosting(const fb200_params* prm, const fb200_inputs* in) {
                                   "frosting->n_bg, sh_rest <= 15)%s");
     if (prm->sh_degree < 0 || prm->sh_degree > 3 || (prm->sh_degree + 1) * (prm->sh_degree + 1) > prm->sh_coeffs)
         return fail(FB200_EINVAL, "sh_degree / sh_coeffs inconsistent%s");
-    if ((reinterpret_cast<uintptr_t>(fp->d_quats) & 15) || (reinterpret_cast<uintptr_t>(fp->d_bary_logits) & 7))
-        return fail(FB200_EINVAL, "frosting mode: quats must be 16-byte aligned, bary logits 8-byte aligned%s");
     if (prm->extra) return fail(FB200_EINVAL, "frosting mode: extra feature channels are not supported%s");
     return FB200_OK;
 }
@@ -371,14 +386,7 @@ int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_
     // there), dL/dcov3D on the scale/rotation path, dL/dscales + dL/drotations on the precomputed-covariance path
     const fb200_frosting_grads* fg = grads->frosting;
     if (in->frosting) {
-        if (!fg) return fail(FB200_EINVAL, "frosting mode: fb200_grads.frosting missing%s");
-        if (prm->P > 0 && (!fg->d_bary_logits || !fg->d_opacity_logits || !fg->d_log_scales || !fg->d_quats || !fg->d_sh_dc ||
-                           (in->frosting->sh_rest > 0 && !fg->d_sh_rest) ||
-                           ((fg->d_inner_verts == nullptr) != (fg->d_outer_verts == nullptr))))
-            return fail(FB200_EINVAL, "frosting mode: parameter-gradient pointers missing%s");
-        if ((reinterpret_cast<uintptr_t>(fg->d_quats) & 15) || (reinterpret_cast<uintptr_t>(fg->d_bary_logits) & 7))
-            return fail(FB200_EINVAL, "frosting mode: dL/dquats must be 16-byte aligned, dL/dbary 8-byte aligned%s");
-        if ((rc = check_background_grads(in->frosting, fg)) != FB200_OK) return rc;
+        if ((rc = check_frosting_grads(in->frosting, fg)) != FB200_OK) return rc;
     } else if (fg) {
         return fail(FB200_EINVAL, "fb200_grads.frosting given without fb200_inputs.frosting%s");
     } else if (prm->P > 0 && (!grads->d_dL_dmeans2D || !grads->d_dL_dopacity || !grads->d_dL_dmeans3D ||
@@ -473,7 +481,10 @@ int fb200_frosting_attributes(const fb200_frosting_params* fp, float* d_means3D,
     const bool rows = (int64_t)fp->P + fp->n_bg > 0;
     if (rows && (!d_means3D || !d_opacities || !d_scales || !d_rotations || !d_shs))
         return fail(FB200_EINVAL, "frosting_attributes: missing output pointer%s");
-    if (rows && (reinterpret_cast<uintptr_t>(d_rotations) & 15))
+    // mesh rows of 16 SH coefficients are stored as twelve float4
+    if (fp->P > 0 && fp->sh_rest == 15 && misaligned(d_shs, 16))
+        return fail(FB200_EINVAL, "frosting_attributes: shs must be 16-byte aligned when sh_rest == 15%s");
+    if (rows && misaligned(d_rotations, 16))
         return fail(FB200_EINVAL, "frosting_attributes: rotations must be 16-byte aligned%s");
     return check(launch_frosting_attr_fwd(*fp, d_means3D, d_opacities, d_scales, d_rotations, d_shs,
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes");
@@ -485,17 +496,15 @@ int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const fl
                                        const fb200_frosting_grads* grads, void* stream) {
     int rc = check_frosting(fp);
     if (rc != FB200_OK) return rc;
-    if (!grads) return fail(FB200_EINVAL, "frosting_attributes_backward: null grads%s");
+    if ((rc = check_frosting_grads(fp, grads)) != FB200_OK) return rc;
     const bool rows = (int64_t)fp->P + fp->n_bg > 0;
     if (rows && (!d_g_means3D || !d_g_opacities || !d_g_scales || !d_g_rotations || !d_g_shs))
         return fail(FB200_EINVAL, "frosting_attributes_backward: missing upstream gradient pointer%s");
-    if (rows && (reinterpret_cast<uintptr_t>(d_g_rotations) & 15))
+    // mesh rows of 16 SH coefficients are read as twelve float4
+    if (fp->P > 0 && fp->sh_rest == 15 && misaligned(d_g_shs, 16))
+        return fail(FB200_EINVAL, "frosting_attributes_backward: dL/dshs must be 16-byte aligned when sh_rest == 15%s");
+    if (rows && misaligned(d_g_rotations, 16))
         return fail(FB200_EINVAL, "frosting_attributes_backward: dL/drotations must be 16-byte aligned%s");
-    if (fp->P > 0 && (!grads->d_bary_logits || !grads->d_opacity_logits || !grads->d_log_scales || !grads->d_quats ||
-                      !grads->d_sh_dc || (fp->sh_rest > 0 && !grads->d_sh_rest) ||
-                      ((grads->d_inner_verts == nullptr) != (grads->d_outer_verts == nullptr))))
-        return fail(FB200_EINVAL, "frosting_attributes_backward: missing pointer%s");
-    if ((rc = check_background_grads(fp, grads)) != FB200_OK) return rc;
     return check(launch_frosting_attr_bwd(*fp, d_g_means3D, d_g_opacities, d_g_scales, d_g_rotations, d_g_shs, *grads,
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes_backward");
 }
@@ -531,14 +540,21 @@ int fb200_frosting_edit_shell(const fb200_frosting_edit* e, void* stream) {
     return check(launch_frosting_edit_shell(*e, static_cast<cudaStream_t>(stream)), "frosting_edit_shell");
 }
 
-static int check_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
-                                 const float* d_campos, const float* d_orig_quats, float* d_means3D,
-                                 float* d_opacities, float* d_scales, float* d_rotations, float* d_colors) {
+// an edit and the parameter block it adapts: each valid, over the same base mesh
+static int check_edit_block(const fb200_frosting_edit* e, const fb200_frosting_params* fp) {
     int rc = check_edit(e);
     if (rc != FB200_OK) return rc;
     if ((rc = check_frosting(fp)) != FB200_OK) return rc;
     if (fp->n_faces != e->n_faces || fp->n_verts != e->n_verts)
         return fail(FB200_EINVAL, "frosting_edit: the parameter block's mesh does not match the edit's%s");
+    return FB200_OK;
+}
+
+static int check_edit_attributes(const fb200_frosting_edit* e, const fb200_frosting_params* fp, int32_t sh_degree,
+                                 const float* d_campos, const float* d_orig_quats, float* d_means3D,
+                                 float* d_opacities, float* d_scales, float* d_rotations, float* d_colors) {
+    int rc = check_edit_block(e, fp);
+    if (rc != FB200_OK) return rc;
     if (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > fp->sh_rest + 1)
         return fail(FB200_EINVAL, "frosting_edit: sh_degree needs (sh_degree + 1)^2 <= sh_rest + 1 <= 16%s");
     const bool rows = (int64_t)fp->P + fp->n_bg > 0;
@@ -571,11 +587,8 @@ static int check_edit_complex(const fb200_frosting_edit* e, const fb200_frosting
 
 int fb200_frosting_edit_complex_capture(const fb200_frosting_edit* e, const fb200_frosting_params* fp, float* d_cell_T,
                                         float* d_canonical, uint32_t* d_n_singular, void* stream) {
-    int rc = check_edit(e);
+    int rc = check_edit_block(e, fp);
     if (rc != FB200_OK) return rc;
-    if ((rc = check_frosting(fp)) != FB200_OK) return rc;
-    if (fp->n_faces != e->n_faces || fp->n_verts != e->n_verts)
-        return fail(FB200_EINVAL, "frosting_edit: the parameter block's mesh does not match the edit's%s");
     if ((rc = check_edit_complex(e, fp, d_cell_T, d_canonical)) != FB200_OK) return rc;
     if (!d_n_singular) return fail(FB200_EINVAL, "frosting_edit_complex: missing singular-cell counter%s");
     return check(launch_frosting_edit_complex_capture(*e, *fp, d_cell_T, d_canonical, d_n_singular,

@@ -20,7 +20,8 @@ import torch
 
 from . import _lib
 from . import rasterizer as R
-from .frosting_render import background_params, _p, _params_block, _stream
+from ._lib import ptr, stream
+from .frosting_render import FrostingBlock
 
 RESCALING = {"median": _lib.RESCALE_MEDIAN, "triangle": _lib.RESCALE_TRIANGLE}
 
@@ -88,13 +89,13 @@ class FrostingEdit:
     def _struct(self, base_verts, threshold, inner, outer):
         return _lib.FrostingEdit(
             n_verts=self.n_verts, n_faces=self.n_faces, rescaling=RESCALING[self.rescaling], n_edited=self.n_edited,
-            deformation_threshold=float(threshold), d_base_verts=_p(base_verts), d_faces=_p(self.faces),
-            d_inner_dist=_p(self.inner_dist), d_outer_dist=_p(self.outer_dist), d_edition_mask=_p(self.edition_mask),
-            d_verts_edition_mask=_p(self.verts_edition_mask), d_vf_offsets=_p(self.vf_offsets),
-            d_vf_faces=_p(self.vf_faces), d_ref_quats=_p(self.ref_quats), d_ref_dists=_p(self.ref_dists),
-            d_ref_median=_p(self.ref_median), d_dists=_p(self.dists), d_face_normals=_p(self.face_normals),
-            d_rel_quats=_p(self.rel_quats), d_face_factor=_p(self.face_factor), d_face_keep=_p(self.face_keep),
-            d_factor=_p(self.factor), d_select=_p(self._select), d_inner_verts=_p(inner), d_outer_verts=_p(outer))
+            deformation_threshold=float(threshold), d_base_verts=ptr(base_verts), d_faces=ptr(self.faces),
+            d_inner_dist=ptr(self.inner_dist), d_outer_dist=ptr(self.outer_dist), d_edition_mask=ptr(self.edition_mask),
+            d_verts_edition_mask=ptr(self.verts_edition_mask), d_vf_offsets=ptr(self.vf_offsets),
+            d_vf_faces=ptr(self.vf_faces), d_ref_quats=ptr(self.ref_quats), d_ref_dists=ptr(self.ref_dists),
+            d_ref_median=ptr(self.ref_median), d_dists=ptr(self.dists), d_face_normals=ptr(self.face_normals),
+            d_rel_quats=ptr(self.rel_quats), d_face_factor=ptr(self.face_factor), d_face_keep=ptr(self.face_keep),
+            d_factor=ptr(self.factor), d_select=ptr(self._select), d_inner_verts=ptr(inner), d_outer_verts=ptr(outer))
 
     def _shell(self, base_verts, threshold):
         if base_verts.shape != (self.n_verts, 3):
@@ -103,7 +104,7 @@ class FrostingEdit:
         inner, outer = torch.empty((self.n_verts, 3), **o), torch.empty((self.n_verts, 3), **o)
         st = self._struct(base_verts, threshold, inner, outer)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().fb200_frosting_edit_shell(C.byref(st), _stream(self.device)))
+            _lib.check(_lib.lib().fb200_frosting_edit_shell(C.byref(st), stream(self.device)))
         return st, inner, outer
 
     def shell(self, base_verts, deformation_threshold=2.0):
@@ -112,16 +113,14 @@ class FrostingEdit:
         return inner, outer
 
     def _block(self, params, inner, outer, face_visible):
-        fp, keep, _, dev = _params_block(params["bary_logits"], params["opacity_logits"], params["log_scales"],
-                                         params["quats"], params["sh_dc"], params["sh_rest"], inner, outer, self.cells,
-                                         self.faces, face_visible, background_params(params))
-        if fp.P != self.cells.numel():
+        blk = FrostingBlock(params, dict(inner=inner, outer=outer, cells=self.cells, faces=self.faces), face_visible)
+        if blk.n_mesh != self.cells.numel():
             raise ValueError("params have a different number of mesh-bound Gaussians than the edit's cells")
-        return fp, keep, dev
+        return blk
 
-    def _launch_attributes(self, st, fp, sh_degree, cp, oq, outs, stream):
-        _lib.check(_lib.lib().fb200_frosting_edit_attributes(C.byref(st), C.byref(fp), int(sh_degree), _p(cp), _p(oq),
-                                                              *(_p(t) for t in outs), stream))
+    def _launch_attributes(self, st, blk, sh_degree, cp, oq, outs):
+        _lib.check(_lib.lib().fb200_frosting_edit_attributes(C.byref(st), C.byref(blk.fp), int(sh_degree), ptr(cp),
+                                                              ptr(oq), *(ptr(t) for t in outs), stream(blk.device)))
 
     @torch.no_grad()
     def attributes(self, params, base_verts, campos, sh_degree, orig_quats=None, deformation_threshold=2.0,
@@ -133,8 +132,8 @@ class FrostingEdit:
         culled faces are skipped (zero rows)."""
         base_verts = R._f32c(base_verts, self.device, "base_verts")
         st, inner, outer = self._shell(base_verts, deformation_threshold)
-        fp, keep, dev = self._block(params, inner, outer, face_visible)
-        rows = fp.P + fp.n_bg
+        blk = self._block(params, inner, outer, face_visible)
+        dev, rows = blk.device, blk.rows
         oq = None
         if orig_quats is not None:
             oq = R._f32c(orig_quats, dev, "orig_quats")
@@ -146,8 +145,7 @@ class FrostingEdit:
         means3D, opac, scales = alloc((rows, 3), **o), alloc((rows, 1), **o), alloc((rows, 3), **o)
         rots, colors = alloc((rows, 4), **o), alloc((rows, 3), **o)
         with torch.cuda.device(dev):
-            self._launch_attributes(st, fp, sh_degree, cp, oq, (means3D, opac, scales, rots, colors), _stream(dev))
-        del keep
+            self._launch_attributes(st, blk, sh_degree, cp, oq, (means3D, opac, scales, rots, colors))
         return dict(means3D=means3D, opacities=opac, scales=scales, rotations=rots, colors_precomp=colors,
                     inner=inner, outer=outer)
 
@@ -173,25 +171,25 @@ class FrostingEditComplex(FrostingEdit):
     def _capture(self, base_verts):
         # after the reference shell, d_dists / d_factor[0] hold the reference distances and median the cells scale by
         st, inner, outer = super()._capture(base_verts)
-        fp, keep, dev = self._block(self._capture_params, inner, outer, None)
+        blk = self._block(self._capture_params, inner, outer, None)
+        dev = blk.device
         o = dict(dtype=torch.float32, device=dev)
         self.cell_T = torch.zeros((self.n_faces, 3, 3), **o)
-        self.canonical = torch.empty((fp.P, 3, 3), **o)
+        self.canonical = torch.empty((blk.n_mesh, 3, 3), **o)
         n_singular = torch.empty((1,), dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().fb200_frosting_edit_complex_capture(
-                C.byref(st), C.byref(fp), _p(self.cell_T), _p(self.canonical), _p(n_singular), _stream(dev)))
-        del keep
+                C.byref(st), C.byref(blk.fp), ptr(self.cell_T), ptr(self.canonical), ptr(n_singular), stream(dev)))
         n = int(n_singular.item())                      # the one host read-back, at capture only
         if n:
             raise ValueError(f"{n} edited Gaussian(s) sit on faces whose cell transformation is singular even after "
                              "the fix-up (degenerate edited faces): their canonical transforms are undefined")
         return st, inner, outer
 
-    def _launch_attributes(self, st, fp, sh_degree, cp, oq, outs, stream):
+    def _launch_attributes(self, st, blk, sh_degree, cp, oq, outs):
         _lib.check(_lib.lib().fb200_frosting_edit_attributes_complex(
-            C.byref(st), C.byref(fp), int(sh_degree), _p(cp), _p(oq), _p(self.canonical), _p(self.cell_T),
-            *(_p(t) for t in outs), stream))
+            C.byref(st), C.byref(blk.fp), int(sh_degree), ptr(cp), ptr(oq), ptr(self.canonical), ptr(self.cell_T),
+            *(ptr(t) for t in outs), stream(blk.device)))
 
 
 @torch.no_grad()

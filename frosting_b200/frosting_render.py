@@ -20,8 +20,13 @@ fewer kernels and ~1 GB less HBM traffic than attribute kernel + rasterizer + at
 Background Gaussians (Frosting's default for real scenes, frosting_model.py:564-591, :801-876): the six `bg_*` keys of
 `params` (BG_KEYS) add free Gaussians after the mesh-bound ones, in the same frame and the same kernels.  They skip the
 occlusion lookup (`render_mask`'s trailing ones, :1571-1576); radii cover all n_mesh + n_bg Gaussians and the backward
-returns the background parameters' gradients too.  `frosting_render_two_step` keeps the attribute-kernel route (tests
-compare the two).
+returns the background parameters' gradients too.
+
+The stand-alone attribute kernels (csrc/frosting_attr.cu, SURVEY.md row a20) serve `frosting_attributes_fused` -- the
+rasterizer inputs of Frosting's properties from one kernel, the parameter gradients from one backward kernel -- and
+`frosting_render_two_step`, which keeps the attribute-kernel route (tests compare the two).
+
+`FrostingBlock` owns the parameter block (fb200_frosting_params) all of them, the edit and the texture bake launch with.
 """
 import ctypes as C
 
@@ -29,127 +34,151 @@ import torch
 
 from . import _lib
 from . import rasterizer as R
-from ._lib import FrostingParams, FrostingGrads
+from ._lib import FrostingParams, FrostingGrads, ptr, stream
 
 MESH_KEYS = ("bary_logits", "opacity_logits", "log_scales", "quats", "sh_dc", "sh_rest")
 # Frosting's _bg_points, _bg_opacities, _bg_scales, _bg_quaternions, _bg_sh_coordinates_dc / _rest, in this order
 BG_KEYS = ("bg_points", "bg_opacity_logits", "bg_log_scales", "bg_quats", "bg_sh_dc", "bg_sh_rest")
+SHELL_KEYS = ("inner", "outer", "cells", "faces")
 
 
-def _p(t):
-    return None if t is None or t.numel() == 0 else C.c_void_p(t.data_ptr())
-
-
-def background_params(params):
-    """The six background tensors of `params` in BG_KEYS order, or None when it has none (all six or none)."""
+def _has_background(params):
+    """Whether `params` holds the six background tensors (all six or none)."""
     have = [k in params for k in BG_KEYS]
-    if not any(have):
-        return None
-    if not all(have):
+    if any(have) and not all(have):
         raise ValueError(f"background Gaussians need all of {BG_KEYS}")
-    return tuple(params[k] for k in BG_KEYS)
+    return all(have)
 
 
-def _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces, face_visible,
-                  bg, mask=None):
-    """fb200_frosting_params over the whole model: the mesh parameters and shell, the optional culling inputs and the
-    background parameters `bg` (BG_KEYS order; empty: none).  Returns it, the mesh-side tensors it points into
-    (parameters, inner, outer, cells, faces, face_visible, mask), the background ones (None: none) and the device."""
-    if not bary_logits.is_cuda:
-        raise RuntimeError("frosting_b200 runs on CUDA tensors only (no CPU fallback)")
-    dev = bary_logits.device
-    t = [R._f32c(x, dev, "frosting parameter") for x in (bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer)]
-    bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer = t
-    cells = cells.to(device=dev, dtype=torch.int64).contiguous()
-    faces = faces.to(device=dev, dtype=torch.int32).contiguous()
-    fv = None if face_visible is None else face_visible.to(device=dev, dtype=torch.uint8).contiguous()
-    m = None if mask is None else mask.to(device=dev, dtype=torch.uint8).contiguous()
-    P, Rn = bary_logits.shape[0], sh_rest.shape[1]
-    bg_keep = tuple(R._f32c(x, dev, "background parameter") for x in bg) if bg else None
-    b = bg_keep or (None,) * 6
-    n_bg = 0 if bg_keep is None else b[0].shape[0]
-    if bg_keep is not None and (b[0].shape != (n_bg, 3) or b[5].shape != (n_bg, Rn, 3) or
-                                any(x.shape[0] != n_bg for x in b)):
-        raise RuntimeError("background parameters must be [n,3], [n], [n,3], [n,4], [n,1,3], [n,M-1,3] with the mesh "
-                           "block's M")
-    fp = FrostingParams(P=P, n_verts=inner.shape[0], n_faces=faces.shape[0], sh_rest=Rn,
-                        d_bary_logits=_p(bary_logits), d_cells=_p(cells), d_faces=_p(faces),
-                        d_inner_verts=_p(inner), d_outer_verts=_p(outer), d_opacity_logits=_p(opacity_logits),
-                        d_log_scales=_p(log_scales), d_quats=_p(quats), d_sh_dc=_p(sh_dc), d_sh_rest=_p(sh_rest),
-                        d_mask=_p(m), d_face_visible=_p(fv), d_radii=None,
-                        n_bg=n_bg, d_bg_points=_p(b[0]), d_bg_opacity_logits=_p(b[1]), d_bg_log_scales=_p(b[2]),
-                        d_bg_quats=_p(b[3]), d_bg_sh_dc=_p(b[4]), d_bg_sh_rest=_p(b[5]))
-    keep = (bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces, fv, m)
-    return fp, keep, bg_keep, dev
+class FrostingBlock:
+    """fb200_frosting_params over a whole model, and every tensor it points into.
 
+    `params` / `mesh`: the dicts of `scenes.frosting_layer` (the background keys BG_KEYS optional); `face_visible` [F] and
+    `mask` [n_mesh]: optional culling inputs.  The tensors are kept, converted for the kernels, in `tensors` under the
+    struct's field names (without `d_`), so the struct `fp` and the memory it points to live and die together.  The frame
+    has `rows` = `n_mesh` mesh-bound Gaussians and `n_bg` background ones after them.
 
-def _grads_block(d, d_in, d_out, bd):
-    """fb200_frosting_grads over the six mesh parameter gradients, the shell vertices' and the background ones (bd:
-    six tensors, or None without background Gaussians)."""
-    b = bd or (None,) * 6
-    return FrostingGrads(d_bary_logits=_p(d[0]), d_inner_verts=_p(d_in), d_outer_verts=_p(d_out),
-                         d_opacity_logits=_p(d[1]), d_log_scales=_p(d[2]), d_quats=_p(d[3]), d_sh_dc=_p(d[4]),
-                         d_sh_rest=_p(d[5]), d_bg_points=_p(b[0]), d_bg_opacity_logits=_p(b[1]),
-                         d_bg_log_scales=_p(b[2]), d_bg_quats=_p(b[3]), d_bg_sh_dc=_p(b[4]), d_bg_sh_rest=_p(b[5]))
+    The autograd Functions below take the block's inputs as `leaves(params, mesh, *call)`: the six mesh parameters, the
+    shell (inner, outer), cells, faces, the Function's N_CALL per-call arguments, then the six background parameters;
+    `autograd_grads` returns the gradients in that order."""
 
+    N_CALL = 3
 
-def _grad_targets(sink, keep, dev, radii, zero_rows, bg_keep=None):
-    """The six parameter-gradient tensors -- and with background Gaussians their six -- : the caller's sink (the
-    optimizer's slab) or fresh ones.  Returns (mesh list, background list or None)."""
-    bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest = keep[:6]
-    P, Rn = bary_logits.shape[0], sh_rest.shape[1]
-    o = dict(dtype=torch.float32, device=dev)
-    if sink is not None:
-        if hasattr(sink, "sink_once"):
-            sink.sink_once(MESH_KEYS + (BG_KEYS if bg_keep is not None else ()))
-        out = [sink[n] for n in MESH_KEYS]
-        bout = [sink[n] for n in BG_KEYS] if bg_keep is not None else None
-        for tt, ref in zip(out + (bout or []), list(keep[:6]) + list(bg_keep or ())):
-            if tt.numel() != ref.numel() or not tt.is_contiguous() or tt.dtype != torch.float32 or tt.device != dev:
-                raise RuntimeError("grad_sink tensors must be contiguous fp32 CUDA tensors shaped like the parameters")
-        if zero_rows:
-            if getattr(sink, "accepts_row_radii", False):
-                # rows with radii <= 0 stay unwritten; the consumer (FrostingAdam's step) treats them as zero rows.  The
-                # background groups have no row structure there: they are zero-filled and stay dense
-                sink.rows_from(radii if bout is None else radii[:P], MESH_KEYS)
-                for tt in bout or ():
-                    tt.zero_()
-            else:
-                for tt in out + (bout or []):
-                    tt.zero_()
-        return out, bout
-    make = torch.zeros if zero_rows else torch.empty
-    bout = None if bg_keep is None else [make(tuple(t.shape), **o) for t in bg_keep]
-    return [make((P, 6), **o), make((P,), **o), make((P, 3), **o), make((P, 4), **o), make((P, 1, 3), **o),
-            make((P, Rn, 3), **o)], bout
+    def __init__(self, params, mesh, face_visible=None, mask=None):
+        self.has_bg = _has_background(params)
+        if not params["bary_logits"].is_cuda:
+            raise RuntimeError("frosting_b200 runs on CUDA tensors only (no CPU fallback)")
+        dev = self.device = params["bary_logits"].device
+        t = {k: R._f32c(params[k], dev, "frosting parameter") for k in MESH_KEYS}
+        t["inner_verts"] = R._f32c(mesh["inner"], dev, "frosting parameter")
+        t["outer_verts"] = R._f32c(mesh["outer"], dev, "frosting parameter")
+        t["cells"] = mesh["cells"].to(device=dev, dtype=torch.int64).contiguous()
+        t["faces"] = mesh["faces"].to(device=dev, dtype=torch.int32).contiguous()
+        t["face_visible"] = None if face_visible is None else face_visible.to(device=dev, dtype=torch.uint8).contiguous()
+        t["mask"] = None if mask is None else mask.to(device=dev, dtype=torch.uint8).contiguous()
+        self.n_mesh, Rn = t["bary_logits"].shape[0], t["sh_rest"].shape[1]
+        self.n_bg = 0
+        if self.has_bg:
+            t.update({k: R._f32c(params[k], dev, "background parameter") for k in BG_KEYS})
+            n = self.n_bg = t["bg_points"].shape[0]
+            if t["bg_points"].shape != (n, 3) or t["bg_sh_rest"].shape != (n, Rn, 3) or \
+                    any(t[k].shape[0] != n for k in BG_KEYS):
+                raise RuntimeError("background parameters must be [n,3], [n], [n,3], [n,4], [n,1,3], [n,M-1,3] with the "
+                                   "mesh block's M")
+        self.rows = self.n_mesh + self.n_bg
+        self.tensors = t
+        self.vert_grad = mesh["inner"].requires_grad or mesh["outer"].requires_grad
+        self.fp = FrostingParams(P=self.n_mesh, n_verts=t["inner_verts"].shape[0], n_faces=t["faces"].shape[0],
+                                 sh_rest=Rn, n_bg=self.n_bg, **{"d_" + k: ptr(v) for k, v in t.items()})
 
+    @staticmethod
+    def leaves(params, mesh, *call):
+        """autograd's inputs for the block of `params` / `mesh` and a Function's N_CALL per-call arguments `call`."""
+        bg = tuple(params[k] for k in BG_KEYS) if _has_background(params) else ()
+        return tuple(params[k] for k in MESH_KEYS) + tuple(mesh[k] for k in SHELL_KEYS) + call + bg
 
-def _returned(ctx, keep, d, d_in, d_out, bg_keep, bd):
-    """autograd's gradients for (mesh parameters, shell vertices, the five non-differentiable inputs -- cells, faces and
-    three per-call arguments --, background parameters)."""
-    tail = (None,) * 5
-    if bg_keep is not None:
-        tail += (None,) * 6 if ctx.sink is not None else (bd[0], bd[1].view_as(bg_keep[1])) + tuple(bd[2:])
-    if ctx.sink is not None:
-        return (None, None, None, None, None, None, d_in, d_out) + tail
-    d_bary, d_op, d_ls, d_q, d_dc, d_rest = d
-    return (d_bary, d_op.view_as(keep[1]), d_ls, d_q, d_dc, d_rest, d_in, d_out) + tail
+    @staticmethod
+    def split(leaves):
+        """(params, mesh, call) of `leaves(params, mesh, *call)`."""
+        n, s = len(MESH_KEYS), len(MESH_KEYS) + len(SHELL_KEYS)
+        params = dict(zip(MESH_KEYS, leaves[:n]))
+        params.update(zip(BG_KEYS, leaves[s + FrostingBlock.N_CALL:]))
+        return params, dict(zip(SHELL_KEYS, leaves[n:s])), leaves[s:s + FrostingBlock.N_CALL]
 
+    def grad_targets(self, sink, radii=None, zero_rows=False):
+        """fb200_frosting_grads and the tensors it points into, by name: the parameter gradients -- the caller's sink (the
+        optimizer's slab) or fresh tensors -- and the shell's (`inner_verts`, `outer_verts`: None unless the shell takes
+        gradients).  `zero_rows`: the backward writes the rendered rows only (frosting mode) and the others are zero: a
+        sink that understands `row_radii` is told so, anything else is zero-filled."""
+        names = MESH_KEYS + (BG_KEYS if self.has_bg else ())
+        if sink is not None:
+            if hasattr(sink, "sink_once"):
+                sink.sink_once(names)
+            d = {k: sink[k] for k in names}
+            for k in names:
+                tt, ref = d[k], self.tensors[k]
+                if tt.numel() != ref.numel() or not tt.is_contiguous() or tt.dtype != torch.float32 or \
+                        tt.device != self.device or tt.data_ptr() % 16:
+                    raise RuntimeError("grad_sink tensors must be contiguous, 16-byte aligned fp32 CUDA tensors shaped "
+                                       "like the parameters")
+            if zero_rows:
+                if getattr(sink, "accepts_row_radii", False):
+                    # rows with radii <= 0 stay unwritten; the consumer (FrostingAdam's step) treats them as zero rows.
+                    # The background groups have no row structure there: they are zero-filled and stay dense
+                    sink.rows_from(radii[:self.n_mesh] if self.has_bg else radii, MESH_KEYS)
+                    for k in BG_KEYS if self.has_bg else ():
+                        d[k].zero_()
+                else:
+                    for tt in d.values():
+                        tt.zero_()
+        else:
+            make, o = torch.zeros if zero_rows else torch.empty, dict(dtype=torch.float32, device=self.device)
+            P, Rn = self.n_mesh, self.fp.sh_rest
+            d = {k: make(tuple(self.tensors[k].shape), **o) for k in BG_KEYS if self.has_bg}
+            shapes = ((P, 6), (P,), (P, 3), (P, 4), (P, 1, 3), (P, Rn, 3))
+            d.update((k, make(shape, **o)) for k, shape in zip(MESH_KEYS, shapes))
+        d["inner_verts"] = torch.empty_like(self.tensors["inner_verts"]) if self.vert_grad else None
+        d["outer_verts"] = torch.empty_like(self.tensors["outer_verts"]) if self.vert_grad else None
+        return FrostingGrads(**{"d_" + k: ptr(v) for k, v in d.items()}), d
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    def autograd_grads(self, d, sink):
+        """autograd's gradients for `leaves`, from the tensors of `grad_targets`: the parameters' (None when they went to
+        a sink), the shell's, None for cells, faces and the per-call arguments."""
+        def g(k):
+            if sink is not None:
+                return None
+            return d[k].view_as(self.tensors[k]) if k in ("opacity_logits", "bg_opacity_logits") else d[k]
+        bg = tuple(g(k) for k in BG_KEYS) if self.has_bg else ()
+        return tuple(g(k) for k in MESH_KEYS) + (d["inner_verts"], d["outer_verts"]) + (None,) * (2 + self.N_CALL) + bg
+
+    def attributes(self, alloc):
+        """fb200_frosting_attributes: means3D, opacities, scales, rotations, shs of the block's rows, in tensors made by
+        `alloc` (torch.empty / torch.zeros)."""
+        P, o = self.rows, dict(dtype=torch.float32, device=self.device)
+        out = (alloc((P, 3), **o), alloc((P, 1), **o), alloc((P, 3), **o), alloc((P, 4), **o),
+               alloc((P, self.fp.sh_rest + 1, 3), **o))
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().fb200_frosting_attributes(C.byref(self.fp), *(ptr(t) for t in out),
+                                                            stream(self.device)))
+        return out
+
+    def attributes_backward(self, upstream, sink):
+        """fb200_frosting_attributes_backward of the five upstream gradients; returns autograd's gradients."""
+        fg, d = self.grad_targets(sink)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().fb200_frosting_attributes_backward(
+                C.byref(self.fp), *(ptr(g) for g in upstream), C.byref(fg), stream(self.device)))
+        return self.autograd_grads(d, sink)
 
 
 class _FrostingRender(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces,
-                face_visible, rs, sink, *bg):
-        fp, keep, bg_keep, dev = _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner,
-                                               outer, cells, faces, face_visible, bg)
+    def forward(ctx, *leaves):
+        params, mesh, (face_visible, rs, sink) = FrostingBlock.split(leaves)
+        blk = FrostingBlock(params, mesh, face_visible)
         color, radii, call, _ = R._launch_forward(None, None, None, None, None, None, None, rs, None,
-                                                  want_backward=True, frosting=(fp, keep, dev))
-        ctx.call, ctx.sink, ctx.keep, ctx.dev, ctx.bg_keep = call, sink, keep, dev, bg_keep
-        ctx.vert_grad = inner.requires_grad or outer.requires_grad
+                                                  want_backward=True, frosting=blk)
+        ctx.blk, ctx.call, ctx.sink = blk, call, sink
         ctx.save_for_backward(radii)
         ctx.mark_non_differentiable(radii)
         return color, radii
@@ -157,37 +186,26 @@ class _FrostingRender(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_color, _):
         (radii,) = ctx.saved_tensors
-        keep, dev, bg_keep = ctx.keep, ctx.dev, ctx.bg_keep
-        d, bd = _grad_targets(ctx.sink, keep, dev, radii, zero_rows=True, bg_keep=bg_keep)
-        d_in = torch.empty_like(keep[6]) if ctx.vert_grad else None
-        d_out = torch.empty_like(keep[7]) if ctx.vert_grad else None
-        R._launch_backward(ctx.call, radii, g_color, frosting_grads=_grads_block(d, d_in, d_out, bd))
-        return _returned(ctx, keep, d, d_in, d_out, bg_keep, bd)
+        fg, d = ctx.blk.grad_targets(ctx.sink, radii, zero_rows=True)
+        R._launch_backward(ctx.call, radii, g_color, frosting_grads=fg)
+        return ctx.blk.autograd_grads(d, ctx.sink)
 
 
 class _FrostingRenderTwoStep(torch.autograd.Function):
     """Attribute kernel -> rasterizer -> attribute backward (round 2a's route; kept as the cross-check of frosting mode)."""
 
     @staticmethod
-    def forward(ctx, bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner, outer, cells, faces,
-                face_visible, rs, sink, *bg):
-        fp, keep, bg_keep, dev = _params_block(bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest, inner,
-                                               outer, cells, faces, face_visible, bg)
-        fv = keep[10]
-        P, Rn = fp.P + fp.n_bg, fp.sh_rest
-        o = dict(dtype=torch.float32, device=dev)
+    def forward(ctx, *leaves):
+        params, mesh, (face_visible, rs, sink) = FrostingBlock.split(leaves)
+        blk = FrostingBlock(params, mesh, face_visible)
         # rows of occluded Gaussians are never read by preprocess (same lookup): plain empty allocations
-        means3D, opac = torch.empty((P, 3), **o), torch.empty((P, 1), **o)
-        scales, rots, shs = torch.empty((P, 3), **o), torch.empty((P, 4), **o), torch.empty((P, Rn + 1, 3), **o)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().fb200_frosting_attributes(
-                C.byref(fp), _p(means3D), _p(opac), _p(scales), _p(rots), _p(shs), _stream(dev)))
+        means3D, opac, scales, rots, shs = blk.attributes(torch.empty)
+        fv = blk.tensors["face_visible"]
         e = torch.Tensor([])
         color, radii, call, _ = R._launch_forward(
             means3D, shs, e, opac, scales, rots, e, rs, None, want_backward=True,
-            face_visibility=(fv, keep[8]) if fv is not None else None)
-        ctx.fp, ctx.call, ctx.sink, ctx.keep, ctx.dev, ctx.bg_keep = fp, call, sink, keep, dev, bg_keep
-        ctx.vert_grad = inner.requires_grad or outer.requires_grad
+            face_visibility=(fv, blk.tensors["cells"]) if fv is not None else None)
+        ctx.blk, ctx.call, ctx.sink = blk, call, sink
         ctx.save_for_backward(radii)
         ctx.mark_non_differentiable(radii)
         return color, radii
@@ -195,26 +213,31 @@ class _FrostingRenderTwoStep(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_color, _):
         (radii,) = ctx.saved_tensors
-        keep, dev, bg_keep = ctx.keep, ctx.dev, ctx.bg_keep
         (dL_dmeans2D, _c, dL_dopacity, dL_dmeans3D, _cov, dL_dsh, dL_dscales, dL_drotations, _e) = R._launch_backward(
             ctx.call, radii, g_color, sparse_rows=True)
-        d, bd = _grad_targets(ctx.sink, keep, dev, radii, zero_rows=False, bg_keep=bg_keep)
-        d_in = torch.empty_like(keep[6]) if ctx.vert_grad else None
-        d_out = torch.empty_like(keep[7]) if ctx.vert_grad else None
-        fp = ctx.fp
-        fp.d_radii = _p(radii)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().fb200_frosting_attributes_backward(
-                C.byref(fp), _p(dL_dmeans3D), _p(dL_dopacity), _p(dL_dscales), _p(dL_drotations), _p(dL_dsh),
-                C.byref(_grads_block(d, d_in, d_out, bd)), _stream(dev)))
-        return _returned(ctx, keep, d, d_in, d_out, bg_keep, bd)
+        ctx.blk.fp.d_radii = ptr(radii)
+        return ctx.blk.attributes_backward((dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations, dL_dsh), ctx.sink)
 
 
-def _apply(fn, params, mesh, raster_settings, face_visible, grad_sink):
-    bg = background_params(params)
-    return fn.apply(params["bary_logits"], params["opacity_logits"], params["log_scales"], params["quats"],
-                    params["sh_dc"], params["sh_rest"], mesh["inner"], mesh["outer"], mesh["cells"],
-                    mesh["faces"], face_visible, raster_settings, grad_sink, *(bg or ()))
+class _FrostingAttributes(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, *leaves):
+        params, mesh, (face_visible, mask, sink) = FrostingBlock.split(leaves)
+        blk = FrostingBlock(params, mesh, face_visible, mask)
+        # masked rows stay finite for downstream torch code
+        out = blk.attributes(torch.empty if (mask is None and face_visible is None) else torch.zeros)
+        ctx.blk, ctx.sink = blk, sink
+        return out
+
+    @staticmethod
+    def backward(ctx, *upstream):
+        blk = ctx.blk
+        P, o = blk.rows, dict(dtype=torch.float32, device=blk.device)
+        shapes = ((P, 3), (P, 1), (P, 3), (P, 4), (P, blk.fp.sh_rest + 1, 3))
+        upstream = [torch.zeros(s, **o) if g is None else g.contiguous() for g, s in zip(upstream, shapes)]
+        # with a sink the gradients go straight into the optimizer's gradient slab (frosting_b200/optim.py) and autograd
+        # gets None
+        return blk.attributes_backward(upstream, ctx.sink)
 
 
 def frosting_render(params, mesh, raster_settings, face_visible=None, grad_sink=None):
@@ -222,9 +245,25 @@ def frosting_render(params, mesh, raster_settings, face_visible=None, grad_sink=
     camera (None: no occlusion culling).  Returns (color [3,H,W], radii [n_mesh + n_bg]); differentiable w.r.t. the
     parameters -- the background ones (BG_KEYS) included when `params` has them -- and the shell vertices.  `grad_sink`
     (FrostingAdam's `grads`, or a dict of tensors): the parameter gradients are written there instead."""
-    return _apply(_FrostingRender, params, mesh, raster_settings, face_visible, grad_sink)
+    return _FrostingRender.apply(*FrostingBlock.leaves(params, mesh, face_visible, raster_settings, grad_sink))
 
 
 def frosting_render_two_step(params, mesh, raster_settings, face_visible=None, grad_sink=None):
     """The same call through the stand-alone attribute kernels (csrc/frosting_attr.cu)."""
-    return _apply(_FrostingRenderTwoStep, params, mesh, raster_settings, face_visible, grad_sink)
+    return _FrostingRenderTwoStep.apply(*FrostingBlock.leaves(params, mesh, face_visible, raster_settings, grad_sink))
+
+
+def frosting_attributes_fused(params, mesh, mask=None, grad_sink=None, face_visible=None):
+    """The rasterizer inputs of Frosting's properties (`scenes.frosting_attributes`, i.e. frosting_scene/
+    frosting_model.py:713-799): dict(means3D, opacities, scales, rotations, shs), from ONE kernel, with ONE backward kernel
+    that returns the gradients of the learnable parameters and of the shell vertices (inner / outer, scatter-added).
+
+    params / mesh: the dicts of `scenes.frosting_layer` (bary_logits, opacity_logits, log_scales, quats, sh_dc, sh_rest |
+    inner, outer, cells, faces).  `mask` [P] or `face_visible` [F] (cull by face_visible[cells[i]] inside the kernels):
+    masked Gaussians are skipped -- their outputs are zero, their parameter gradients are zero.  `grad_sink` (dict with
+    the parameter names): the backward writes the parameter gradients there (overwriting) instead of returning them to
+    autograd.  With the background keys (BG_KEYS) the outputs cover n_mesh + n_bg Gaussians, background rows last;
+    mask / face_visible apply to the mesh rows only."""
+    means3D, opac, scales, rots, shs = _FrostingAttributes.apply(
+        *FrostingBlock.leaves(params, mesh, face_visible, mask, grad_sink))
+    return dict(means3D=means3D, opacities=opac, scales=scales, rotations=rots, shs=shs)

@@ -5,7 +5,6 @@ frosting_trainers/refine.py:407-409 with frosting_utils/loss_utils.py:17-63, for
 forward kernel (+ a tiny reduction) and one backward kernel behind the C ABI (fb200_l1_dssim_forward/backward).
 `torch_reference(...)` restates the reference's torch code and is the oracle used by the tests.
 """
-import ctypes as C
 import math
 
 import torch
@@ -30,8 +29,7 @@ class _L1DSSIM(torch.autograd.Function):
         loss = torch.empty((1,), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             _lib.check(L.fb200_l1_dssim_forward(p.data_ptr(), g.data_ptr(), Cn, H, W, float(lam), maps.data_ptr(),
-                                                partials.data_ptr(), loss.data_ptr(),
-                                                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                                partials.data_ptr(), loss.data_ptr(), _lib.stream(dev)))
         ctx.save_for_backward(p, g, maps)
         ctx.lam, ctx.shape = float(lam), shape
         return loss.reshape(())
@@ -45,8 +43,7 @@ class _L1DSSIM(torch.autograd.Function):
         dpred = torch.empty_like(p)
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().fb200_l1_dssim_backward(p.data_ptr(), g.data_ptr(), maps.data_ptr(), Cn, H, W, ctx.lam,
-                                                          gl.data_ptr(), dpred.data_ptr(),
-                                                          C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                                          gl.data_ptr(), dpred.data_ptr(), _lib.stream(dev)))
         return dpred.reshape(ctx.shape), None, None
 
 

@@ -12,12 +12,12 @@ pytorch3d is not a dependency: `mesh` is anything with verts_list()/faces_list()
 works) or a (verts, faces) pair; a camera is anything with .full_proj_transform, .image_height,
 .image_width (GSCamera, frosting_scene/cameras.py:142-223) or a wrapper with .gs_cameras.
 """
-import ctypes as C
 from typing import Optional
 
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
 
 
 def _verts_faces(mesh=None, verts=None, faces=None):
@@ -51,12 +51,8 @@ def rasterize_mesh(verts: torch.Tensor, faces: torch.Tensor, full_proj_transform
         face_visible = torch.empty((max(F, 1),), dtype=torch.uint8, device=device)
         scratch = torch.empty((2 * F + 4,), dtype=torch.int32, device=device) if (work_lists and F) else None
         _lib.check(_lib.lib().fb200_mesh_visibility(
-            verts.shape[0], F, C.c_void_p(verts.data_ptr()) if F else None,
-            C.c_void_p(faces.data_ptr()) if F else None, C.c_void_p(proj.data_ptr()), W, H,
-            C.c_void_p(zbuf.data_ptr()), C.c_void_p(pix_to_face.data_ptr()),
-            C.c_void_p(face_visible.data_ptr()), int(bool(mark_last_on_bg)),
-            C.c_void_p(scratch.data_ptr()) if scratch is not None else None,
-            C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
+            verts.shape[0], F, ptr(verts) if F else None, ptr(faces) if F else None, ptr(proj), W, H, ptr(zbuf),
+            ptr(pix_to_face), ptr(face_visible), int(bool(mark_last_on_bg)), ptr(scratch), stream(device)))
     return pix_to_face, face_visible[:F].bool(), zbuf
 
 
@@ -73,9 +69,7 @@ def gaussian_render_mask(face_visible: torch.Tensor, point_cell_indices: torch.T
     mask = torch.empty((n_total,), dtype=torch.uint8, device=device)
     with torch.cuda.device(device):
         _lib.check(_lib.lib().fb200_gaussian_mask_from_faces(
-            n_pts, C.c_void_p(cells.data_ptr()) if n_pts else None, fv.shape[0],
-            C.c_void_p(fv.data_ptr()) if n_pts else None, n_bg, C.c_void_p(mask.data_ptr()),
-            C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
+            n_pts, ptr(cells), fv.shape[0], ptr(fv) if n_pts else None, n_bg, ptr(mask), stream(device)))
     return mask
 
 

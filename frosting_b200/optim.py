@@ -438,7 +438,7 @@ class FrostingAdam:
             dist.all_reduce(loss if loss is not None else self._flag, group=self.group)
         a = self._args()
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().fb200_adam_step(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            _lib.check(_lib.lib().fb200_adam_step(C.byref(a), _lib.stream(dev)))
         if self.world > 1:
             # rendezvous 2: every rank's parameter stores have landed before anyone's next forward
             dist.all_reduce(self._flag, group=self.group)

@@ -13,7 +13,7 @@ One extension: `GaussianRasterizer.forward(..., visibility_mask=None)` takes the
 occlusion mask (frosting_model.py:1564-1576) and drops masked Gaussians inside the preprocess kernel
 instead of boolean-gathering every attribute tensor (frosting_model.py:1578-1586).
 """
-from typing import NamedTuple, Optional
+from typing import NamedTuple
 import ctypes as C
 import os
 import threading
@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import Params, Inputs, Workspace, Grads, Layout
+from ._lib import Params, Inputs, Workspace, Grads, Layout, ptr
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -164,12 +164,6 @@ def _host_state(device) -> _HostState:
     return st
 
 
-def _ptr(t: Optional[torch.Tensor]):
-    if t is None or t.numel() == 0:
-        return None
-    return C.c_void_p(t.data_ptr())
-
-
 def _f32c(t: torch.Tensor, device, name: str) -> torch.Tensor:
     if t.numel() == 0:
         return t
@@ -258,23 +252,23 @@ def _prepare(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_p
                  tanfovx=float(rs.tanfovx), tanfovy=float(rs.tanfovy),
                  scale_modifier=float(rs.scale_modifier), prefiltered=int(bool(rs.prefiltered)),
                  debug=int(bool(rs.debug)) | (2 if NO_CULL else 0), extra=None)
-    inp = Inputs(d_background=_ptr(bg), d_means3D=_ptr(means3D), d_shs=_ptr(sh),
-                 d_colors_precomp=_ptr(colors_precomp), d_opacities=_ptr(opacities), d_scales=_ptr(scales),
-                 d_rotations=_ptr(rotations), d_cov3D_precomp=_ptr(cov3Ds_precomp),
-                 d_viewmatrix=_ptr(view), d_projmatrix=_ptr(proj), d_campos=_ptr(campos), d_visibility=_ptr(vis),
-                 d_point_cells=_ptr(cells) if fvis is not None and cells.numel() else None,
-                 d_face_visible=_ptr(fvis) if fvis is not None and cells.numel() else None,
+    inp = Inputs(d_background=ptr(bg), d_means3D=ptr(means3D), d_shs=ptr(sh),
+                 d_colors_precomp=ptr(colors_precomp), d_opacities=ptr(opacities), d_scales=ptr(scales),
+                 d_rotations=ptr(rotations), d_cov3D_precomp=ptr(cov3Ds_precomp),
+                 d_viewmatrix=ptr(view), d_projmatrix=ptr(proj), d_campos=ptr(campos), d_visibility=ptr(vis),
+                 d_point_cells=ptr(cells) if fvis is not None and cells.numel() else None,
+                 d_face_visible=ptr(fvis) if fvis is not None and cells.numel() else None,
                  n_cell_points=int(cells.numel()) if cells is not None else 0)
     tensors = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, bg, view, proj,
                campos, vis, extra_features, extra_bg, fvis, cells)
     return device, P, W, H, prm, inp, tensors, extra_features, extra_bg
 
 
-def _prepare_frosting(frosting, rs):
-    """Frosting mode (fb200_inputs.frosting): the rasterizer reads the parameter block `fp` itself; no attribute tensors.
-    `frosting` = (fp, keep, device); the frame is fp.P mesh-bound Gaussians and fp.n_bg background ones after them."""
-    fp, keep, device = frosting
-    P, M = int(fp.P) + int(fp.n_bg), int(fp.sh_rest) + 1
+def _prepare_frosting(block, rs):
+    """Frosting mode (fb200_inputs.frosting): the rasterizer reads the parameter block itself; no attribute tensors.
+    `block`: a frosting_render.FrostingBlock; the frame is its rows (mesh-bound Gaussians, then background ones)."""
+    fp, device = block.fp, block.device
+    P, M = block.rows, int(fp.sh_rest) + 1
     H, W = int(rs.image_height), int(rs.image_width)
     bg = _f32c(rs.bg, device, "bg")
     view = _f32c(rs.viewmatrix, device, "viewmatrix")
@@ -284,9 +278,9 @@ def _prepare_frosting(frosting, rs):
                  tanfovx=float(rs.tanfovx), tanfovy=float(rs.tanfovy),
                  scale_modifier=float(rs.scale_modifier), prefiltered=int(bool(rs.prefiltered)),
                  debug=int(bool(rs.debug)) | (2 if NO_CULL else 0), extra=None)
-    inp = Inputs(d_background=_ptr(bg), d_viewmatrix=_ptr(view), d_projmatrix=_ptr(proj), d_campos=_ptr(campos),
+    inp = Inputs(d_background=ptr(bg), d_viewmatrix=ptr(view), d_projmatrix=ptr(proj), d_campos=ptr(campos),
                  n_cell_points=0, frosting=C.addressof(fp))
-    return device, P, W, H, prm, inp, (fp, keep, bg, view, proj, campos), None, None
+    return device, P, W, H, prm, inp, (block, bg, view, proj, campos), None, None
 
 
 def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -322,8 +316,8 @@ def _launch_forward(means3D, sh, colors_precomp, opacities, scales, rotations, c
             out_extra = torch.empty((extra_features.size(1), H, W), dtype=torch.float32, device=device)
             if P == 0:
                 out_extra.copy_(extra_bg.view(-1, 1, 1).expand_as(out_extra))
-            extra = _lib.Extra(channels=extra_features.size(1), d_features=_ptr(extra_features),
-                               d_background=_ptr(extra_bg), d_out=_ptr(out_extra), d_dL_dout=None, d_dL_dfeatures=None)
+            extra = _lib.Extra(channels=extra_features.size(1), d_features=ptr(extra_features),
+                               d_background=ptr(extra_bg), d_out=ptr(out_extra), d_dL_dout=None, d_dL_dfeatures=None)
             prm.extra = C.addressof(extra)
         gb, ib = _sizes(L, P, W, H)
         slab = torch.empty((gb + ib + 128,), dtype=torch.uint8, device=device)   # one allocator call
@@ -429,10 +423,10 @@ def _launch_backward(call: "_Call", radii, grad_out_color, grad_out_extra=None, 
             dL_dextra = torch.empty((P, E), dtype=torch.float32, device=device)
             call.extra.d_dL_dout, call.extra.d_dL_dfeatures = ge.data_ptr(), dL_dextra.data_ptr()
             prm.extra = C.addressof(call.extra)
-        grads = Grads(d_dL_dmeans2D=_ptr(dL_dmeans2D), d_dL_dcolors=_ptr(dL_dcolors),
-                      d_dL_dopacity=_ptr(dL_dopacity), d_dL_dmeans3D=_ptr(dL_dmeans3D),
-                      d_dL_dcov3D=_ptr(dL_dcov3D), d_dL_dsh=_ptr(dL_dsh), d_dL_dscales=_ptr(dL_dscales),
-                      d_dL_drotations=_ptr(dL_drotations), sparse_rows=1 if sparse_rows else 0)
+        grads = Grads(d_dL_dmeans2D=ptr(dL_dmeans2D), d_dL_dcolors=ptr(dL_dcolors),
+                      d_dL_dopacity=ptr(dL_dopacity), d_dL_dmeans3D=ptr(dL_dmeans3D),
+                      d_dL_dcov3D=ptr(dL_dcov3D), d_dL_dsh=ptr(dL_dsh), d_dL_dscales=ptr(dL_dscales),
+                      d_dL_drotations=ptr(dL_drotations), sparse_rows=1 if sparse_rows else 0)
         _lib.check(L.fb200_backward(C.byref(prm), C.byref(call.inp), C.byref(call.ws),
                                     C.c_void_p(radii.data_ptr()) if P > 0 else None,
                                     C.c_void_p(g.data_ptr()), C.byref(grads),
@@ -561,8 +555,7 @@ class GaussianRasterizer(nn.Module):
             present = torch.empty((P,), dtype=torch.bool, device=device)
             with torch.cuda.device(device):
                 _lib.check(_lib.lib().fb200_mark_visible(
-                    P, _ptr(pos), _ptr(view), _ptr(proj), _ptr(present),
-                    C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
+                    P, ptr(pos), ptr(view), ptr(proj), ptr(present), _lib.stream(device)))
         return present
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,

@@ -16,7 +16,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .frosting_render import _p, _stream
+from ._lib import ptr, stream
 
 
 def skin_tables(package, ref_indices, n_verts):
@@ -96,8 +96,8 @@ class FrostingSkin:
         self.reset = torch.linalg.inv(t["rest_t"].to(self.device)).contiguous()
         self._st = _lib.FrostingSkin(
             n_rows=self.vert_ids.numel(), n_verts=self.n_verts, n_bones=len(self.bone_names), n_frames=self.n_frames,
-            d_tpose=_p(self.tpose), d_vert_ids=_p(self.vert_ids), d_offsets=_p(self.offsets), d_bones=_p(self.bones),
-            d_weights=_p(self.weights), d_reset=_p(self.reset), d_pose=_p(self.tracks))
+            d_tpose=ptr(self.tpose), d_vert_ids=ptr(self.vert_ids), d_offsets=ptr(self.offsets), d_bones=ptr(self.bones),
+            d_weights=ptr(self.weights), d_reset=ptr(self.reset), d_pose=ptr(self.tracks))
 
     @torch.no_grad()
     def pose(self, i_frame, base_verts):
@@ -110,5 +110,5 @@ class FrostingSkin:
             raise ValueError("the package has no frames")
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().fb200_frosting_skin_pose(C.byref(self._st), int(i_frame) % self.n_frames,
-                                                           _p(base_verts), _stream(self.device)))
+                                                           ptr(base_verts), stream(self.device)))
         return base_verts

@@ -24,7 +24,8 @@ import torch
 
 from . import _lib
 from . import rasterizer as R
-from .frosting_render import MESH_KEYS, _p, _params_block, _stream, background_params
+from ._lib import ptr, stream
+from .frosting_render import FrostingBlock
 from .mesh import rasterize_mesh
 from .rasterizer import GaussianRasterizationSettings
 from .scenes import texture_uv_layout
@@ -46,8 +47,8 @@ def mesh_bary(verts, faces, full_proj_transform, pix_to_face):
     H, W = p2f.shape
     bary = torch.empty((H, W, 3), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().fb200_mesh_barycentrics(verts.shape[0], faces.shape[0], _p(verts), _p(faces), _p(proj),
-                                                      W, H, _p(p2f), _p(bary), _stream(dev)))
+        _lib.check(_lib.lib().fb200_mesh_barycentrics(verts.shape[0], faces.shape[0], ptr(verts), ptr(faces), ptr(proj),
+                                                      W, H, ptr(p2f), ptr(bary), stream(dev)))
     return bary
 
 
@@ -93,11 +94,11 @@ class TextureBaker:
         self.texel_winner = torch.full((T * T,), -1, dtype=torch.int32, device=dev)
         self._st = _lib.Texture(
             n_faces=F, n_points=P, square_size=self.square_size, n_square_per_axis=n, texture_size=T,
-            d_cell_offsets=_p(self.cell_offsets), d_cell_points=_p(self.cell_points), d_sh_dc=_p(self.sh_dc),
-            d_face_sh=_p(self.face_sh), d_face_acc=_p(self.face_acc), d_texel_acc=_p(self.texel_acc),
-            d_face_winner=_p(self.face_winner), d_texel_winner=_p(self.texel_winner))
+            d_cell_offsets=ptr(self.cell_offsets), d_cell_points=ptr(self.cell_points), d_sh_dc=ptr(self.sh_dc),
+            d_face_sh=ptr(self.face_sh), d_face_acc=ptr(self.face_acc), d_texel_acc=ptr(self.texel_acc),
+            d_face_winner=ptr(self.face_winner), d_texel_winner=ptr(self.texel_winner))
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().fb200_texture_face_sh_colours(C.byref(self._st), _stream(dev)))
+            _lib.check(_lib.lib().fb200_texture_face_sh_colours(C.byref(self._st), stream(dev)))
 
     def add_view(self, image, pix_to_face, bary):
         """One view: image [H,W,3] (the render; nan_to_num and clamp(0, 1) are applied in the kernel), pix_to_face
@@ -112,15 +113,15 @@ class TextureBaker:
         if tuple(image.shape) != (H, W, 3) or tuple(bary.shape) != (H, W, 3):
             raise ValueError(f"image and bary must be [{H}, {W}, 3] like pix_to_face")
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().fb200_texture_add_view(C.byref(self._st), _p(image), _p(p2f), _p(bary), W, H,
-                                                         _stream(dev)))
+            _lib.check(_lib.lib().fb200_texture_add_view(C.byref(self._st), ptr(image), ptr(p2f), ptr(bary), W, H,
+                                                         stream(dev)))
 
     def finish(self):
         """(verts_uvs [6n^2,2], faces_uvs [F,3], texture_map [T,T,3]) as TexturesUV receives them."""
         T = self.texture_size
         texture = torch.empty((T, T, 3), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().fb200_texture_finish(C.byref(self._st), _p(texture), _stream(self.device)))
+            _lib.check(_lib.lib().fb200_texture_finish(C.byref(self._st), ptr(texture), stream(self.device)))
         return self.verts_uvs, self.faces_uvs, texture
 
 
@@ -146,12 +147,8 @@ def render_view(params, mesh, raster_settings, face_visible=None):
     count (the two-phase forward: one host wait per view, where the reference's rasterizer blocks too).  The speculated
     capacity of frosting_render can overflow on one view of a camera ring and only reports it at the next call; a bake
     must never take such a frame."""
-    bg = background_params(params)
-    fp, keep, bg_keep, dev = _params_block(*(params[k] for k in MESH_KEYS), mesh["inner"], mesh["outer"], mesh["cells"],
-                                           mesh["faces"], face_visible, bg or ())
     color, _, _, _ = R._launch_forward(None, None, None, None, None, None, None, raster_settings, None, exact=True,
-                                       frosting=(fp, keep, dev))
-    del bg_keep
+                                       frosting=FrostingBlock(params, mesh, face_visible))
     return color
 
 

@@ -87,7 +87,10 @@ typedef struct fb200_params {
  * properties, :1415-1418 and :1487-1514 the cat).  A frame is P + n_bg rows, mesh-bound rows first.  A background row
  * skips the occlusion lookup (it is always a candidate, :1571-1576) and maps its parameters like a mesh row, without the
  * prism cell: position = d_bg_points (used as is), opacity = sigmoid, scales = exp, rotation = normalize, SH row =
- * dc | rest.  n_bg == 0: mesh-bound Gaussians only, the d_bg_* pointers are not read. */
+ * dc | rest.  n_bg == 0: mesh-bound Gaussians only, the d_bg_* pointers are not read.
+ *
+ * Alignment, checked by every entry point that takes the block (FB200_EINVAL otherwise): with P > 0, d_bary_logits
+ * 8-byte, d_quats and (sh_rest > 0) d_sh_rest 16-byte aligned; with n_bg > 0, d_bg_quats 16-byte aligned. */
 typedef struct fb200_frosting_params {
     int32_t P;                       /* mesh-bound Gaussians */
     int32_t n_verts, n_faces;        /* shell base mesh */
@@ -111,16 +114,17 @@ typedef struct fb200_frosting_params {
     const float* d_bg_points;        /* [n_bg,3]     _bg_points */
     const float* d_bg_opacity_logits;/* [n_bg]       _bg_opacities */
     const float* d_bg_log_scales;    /* [n_bg,3]     _bg_scales */
-    const float* d_bg_quats;         /* [n_bg,4]     _bg_quaternions (raw), 16-byte aligned */
+    const float* d_bg_quats;         /* [n_bg,4]     _bg_quaternions (raw) */
     const float* d_bg_sh_dc;         /* [n_bg,1,3]   _bg_sh_coordinates_dc */
     const float* d_bg_sh_rest;       /* [n_bg,M-1,3] _bg_sh_coordinates_rest */
 } fb200_frosting_params;
 
 typedef struct fb200_frosting_grads {      /* fb200_frosting_attributes_backward: all fully written; frosting mode of
                                             * fb200_backward: rows of rendered Gaussians only.  Inner / outer vertex gradients
-                                            * are accumulated (cleared by the call first).  The d_bg_* rows are the
-                                            * background Gaussians': given exactly when n_bg > 0, d_bg_quats 16-byte
-                                            * aligned */
+                                            * are accumulated (cleared by the call first), both or neither.  The six mesh
+                                            * parameter gradients are required when the block's P > 0, each 16-byte
+                                            * aligned (d_sh_rest when sh_rest > 0).  The d_bg_* rows are the background
+                                            * Gaussians': given exactly when n_bg > 0, d_bg_quats 16-byte aligned */
     float* d_bary_logits; float* d_inner_verts; float* d_outer_verts; float* d_opacity_logits;
     float* d_log_scales; float* d_quats; float* d_sh_dc; float* d_sh_rest;
     float* d_bg_points; float* d_bg_opacity_logits; float* d_bg_log_scales; float* d_bg_quats; float* d_bg_sh_dc;
@@ -273,8 +277,8 @@ int fb200_gaussian_mask_from_faces(int32_t n_points, const int64_t* d_point_cell
 
 /* Frosting's attribute construction as stand-alone kernels (structs: above, before fb200_inputs), the cross-check of
  * frosting mode.  Outputs and upstream gradients have P + n_bg rows, background rows last; d_rotations and
- * d_g_rotations 16-byte aligned.  With d_radii the backward writes zeros for a row with radii <= 0 and does not read its
- * upstream rows. */
+ * d_g_rotations 16-byte aligned, d_shs and d_g_shs too when sh_rest == 15.  With d_radii the backward writes zeros for
+ * a row with radii <= 0 and does not read its upstream rows. */
 int fb200_frosting_attributes(const fb200_frosting_params* fp, float* d_means3D /*[P+n_bg,3]*/,
                               float* d_opacities /*[P+n_bg,1]*/, float* d_scales /*[P+n_bg,3]*/,
                               float* d_rotations /*[P+n_bg,4]*/, float* d_shs /*[P+n_bg,M,3]*/, void* stream);

@@ -181,3 +181,45 @@ def test_frosting_layer_without_background_is_unchanged():
     lo, hi = m["verts"].min(0).values, m["verts"].max(0).values
     assert not bool(((p["bg_points"] > lo) & (p["bg_points"] < hi)).all(1).any())
 
+
+
+MESH_GRADS = ("d_bary_logits", "d_opacity_logits", "d_log_scales", "d_quats", "d_sh_dc", "d_sh_rest")
+
+
+def test_attribute_entry_points_reject_bases_the_kernels_cannot_vector_access():
+    """The attribute kernels move sh_rest, shs (sh_rest == 15) and the mesh parameter gradients with 128-bit accesses.
+    Every call also carries a later argument error, so none of them can reach a launch."""
+    L = _lib.lib()
+    _, fp, _, fg, _ = keep = _frame()
+    fp.d_sh_rest = ODD
+    assert L.fb200_frosting_attributes(C.byref(fp), D, D, D, ODD, D, None) == -1 and \
+        "sh_rest 16-byte aligned" in _err(L)
+    fp.d_sh_rest = D
+    assert L.fb200_frosting_attributes(C.byref(fp), D, D, D, ODD, ODD, None) == -1 and \
+        "shs must be 16-byte aligned" in _err(L)
+    assert L.fb200_frosting_attributes_backward(C.byref(fp), D, D, D, ODD, ODD, C.byref(fg), None) == -1 and \
+        "dL/dshs must be 16-byte aligned" in _err(L)
+    for f in MESH_GRADS:
+        setattr(fg, f, ODD)
+        assert L.fb200_frosting_attributes_backward(C.byref(fp), D, None, D, D, D, C.byref(fg), None) == -1 and \
+            "mesh parameter gradients must be 16-byte aligned" in _err(L), f
+        setattr(fg, f, D)
+    del keep
+
+
+def test_frosting_backward_checks_mesh_gradients_against_the_mesh_rows():
+    """fb200_backward in frosting mode takes the attribute backward's gradient contract: with mesh rows their gradients
+    are required and 16-byte aligned; without (background only, what frosting_render passes for an empty mesh block)
+    they may be NULL.  The misaligned dL/drotations behind the frosting checks shows that a call got past them."""
+    L = _lib.lib()
+    prm, fp, inp, fg, grads = keep = _frame()
+    grads.d_dL_drotations = ODD
+    fg.d_sh_dc = ODD
+    assert _bwd(L, prm, inp, grads) == -1 and "mesh parameter gradients must be 16-byte aligned" in _err(L)
+    fg.d_sh_dc = D
+    assert _bwd(L, prm, inp, grads) == -1 and "dL/drotations / dL/dsh rows must be 16-byte aligned" in _err(L)
+    fp.P, prm.P = 0, 5
+    for f in MESH_GRADS:
+        setattr(fg, f, None)
+    assert _bwd(L, prm, inp, grads) == -1 and "dL/drotations / dL/dsh rows must be 16-byte aligned" in _err(L)
+    del keep

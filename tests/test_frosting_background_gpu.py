@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import frosting_b200 as fb
-from frosting_b200 import optim, scenes
+from frosting_b200 import _lib, optim, scenes
 from frosting_b200.frosting_render import BG_KEYS, MESH_KEYS
 from tests.util import rel_err_stats
 
@@ -213,3 +213,20 @@ def test_frosting_adam_with_background_groups_equals_torch_adam(cuda_device):
                                     lr_delay_mult=o.position_lr_delay_mult, max_steps=o.position_lr_max_steps)
     assert fo.param_groups[6]["lr"] == pytest.approx(sched(15_000)) == lr    # the last scheduled group's lr, as the reference
     assert fo.param_groups[0]["lr"] == pytest.approx(np.sqrt(0.005 * 0.00005))
+
+
+def test_misaligned_grad_sink_is_rejected_before_the_backward(cuda_device):
+    """A sink view at an odd element offset is contiguous, but the backward stores gradient rows with 128-bit accesses:
+    it is refused before the library is called."""
+    dev = cuda_device
+    cam, params, mesh, _ = _layer(dev, 200, 120, 3001, 500, 500, occl=False)
+    rs = scenes.settings_for(cam, 3, device=dev)
+    p, m = _leaves(params, mesh)
+    sink = {k: torch.zeros_like(v) for k, v in params.items()}
+    sink["quats"] = torch.zeros(params["quats"].numel() + 1, device=dev)[1:].view_as(params["quats"])
+    assert sink["quats"].is_contiguous() and sink["quats"].data_ptr() % 16
+    color, _ = fb.frosting_render(p, m, rs, grad_sink=sink)
+    launches = _lib.kernel_launches()
+    with pytest.raises(RuntimeError, match="16-byte aligned"):
+        color.sum().backward()
+    assert _lib.kernel_launches() == launches

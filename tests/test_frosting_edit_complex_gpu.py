@@ -220,3 +220,19 @@ SIMPLE_EDIT_DIGEST = "da758fb014700342a6327de2b2443c4668cd744925e5afe76356843679
 
 def test_simple_adaptation_outputs_are_unchanged():
     assert simple_edit_digest() == SIMPLE_EDIT_DIGEST
+
+
+def test_background_views_give_the_contiguous_frame(cuda_device):
+    """Non-contiguous background parameters, at the capture and per frame, give the contiguous call's tables and frame."""
+    from tests.test_frosting_edit_gpu import strided
+    g, params = golden_case("median_full_bg_d3")
+    params = {k: v.to(DEV) for k, v in params.items()}
+    views = {k: strided(v) if k.startswith("bg_") else v for k, v in params.items()}
+    assert not views["bg_quats"].is_contiguous()
+    (edit, t), (edit_v, _) = _edit_from_golden(g, params), _edit_from_golden(g, views)
+    assert torch.equal(edit.canonical, edit_v.canonical) and torch.equal(edit.cell_T, edit_v.cell_T)
+    a = edit.attributes(params, t("verts"), t("campos"), int(g["sh_degree"]), orig_quats=t("orig_quats"))
+    b = edit_v.attributes(views, t("verts"), t("campos"), int(g["sh_degree"]), orig_quats=t("orig_quats"))
+    for k in a:
+        assert torch.equal(a[k], b[k]), k
+    assert torch.equal(edit.cell_T, edit_v.cell_T)

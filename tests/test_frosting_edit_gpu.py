@@ -140,3 +140,22 @@ def test_face_visible_culling_matches_mask_route():
     assert int(culled.sum()) > 0 and bool((radii[culled] == 0).all())
     assert torch.equal(radii, radii_m)
     assert torch.equal(img, img_m)
+
+
+def strided(x):
+    """The values of `x` as a non-contiguous view."""
+    return torch.stack([x, torch.zeros_like(x)], -1)[..., 0]
+
+
+@pytest.mark.parametrize("name", ["median_full_bg_d3", "triangle_full_bg_d3"])
+def test_background_views_give_the_contiguous_frame(cuda_device, name):
+    """Non-contiguous background parameters are copied for the kernel; the copies must outlive its launch."""
+    g, params = golden_case(name)
+    params = {k: v.to(DEV) for k, v in params.items()}
+    views = {k: strided(v) if k.startswith("bg_") else v for k, v in params.items()}
+    assert not views["bg_points"].is_contiguous()
+    edit, t = _edit_from_golden(g)
+    a = edit.attributes(params, t("verts"), t("campos"), int(g["sh_degree"]), orig_quats=t("orig_quats"))
+    b = edit.attributes(views, t("verts"), t("campos"), int(g["sh_degree"]), orig_quats=t("orig_quats"))
+    for k in a:
+        assert torch.equal(a[k], b[k]), k
