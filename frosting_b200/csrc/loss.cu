@@ -8,7 +8,8 @@
 // 1080p; here: one forward kernel (separable convolution in shared memory, SSIM map, L1 term, per-block loss
 // partials, three derivative maps), one tiny deterministic reduction, one backward kernel (separable
 // convolution of the derivative maps + the L1 sign term).  Tolerance-level arithmetic (the reference convolves
-// with the 2-D outer-product window; the separable form differs by float rounding).
+// with the 2-D outer-product window; the separable form differs by float rounding): tests/test_loss_f64_gpu.py holds
+// it to no worse than the reference's float32 arithmetic, both measured against float64.
 #include "common.cuh"
 
 namespace fb200 {
@@ -64,11 +65,16 @@ l1_dssim_fwd_kernel(const float* __restrict__ pred, const float* __restrict__ gt
     float term = 0.f;
     if (x < W && y < H) {
         const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
-        const float mu1_sq = mu1 * mu1, mu2_sq = mu2 * mu2, mu12 = mu1 * mu2;
+        // Rounded products, as the reference's separate torch ops.  In flat regions sigma^2 = E[x^2] - mu^2 cancels
+        // down to ~C2, and a contraction of s1 and s2 into FMAs but not s12 (mu12 is also needed for A) would make
+        // B != D for identical images: SSIM off 1 by up to ulp(mu^2) / C2 ~ 7e-5 over a whole white background.
+        const float mu1_sq = __fmul_rn(mu1, mu1), mu2_sq = __fmul_rn(mu2, mu2), mu12 = __fmul_rn(mu1, mu2);
         const float s1 = exx - mu1_sq, s2 = eyy - mu2_sq, s12 = exy - mu12;
         const float A = 2.f * mu12 + C1, B = 2.f * s12 + C2, Cc = mu1_sq + mu2_sq + C1, D = s1 + s2 + C2;
         const float inv = 1.0f / (Cc * D);
-        const float ssim = A * B * inv;
+        // divided, as the reference does: identical windows give exactly 1 (A * B * inv can miss it by an ulp, a bias
+        // that sums over every pixel where the prediction matches the ground truth)
+        const float ssim = (A * B) / (Cc * D);
         // derivatives of the SSIM value w.r.t. mu1, E[x^2], E[xy] (E[.] held independent)
         const float dA = 2.f * mu2, dB = -2.f * mu2, dC = 2.f * mu1, dD = -2.f * mu1;
         const float d_mu1 = (dA * B + A * dB) * inv - ssim * (dC * D + Cc * dD) * inv;
