@@ -31,7 +31,7 @@ EXPORTED = [
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
 NUM_STAGES = 5
-ABI_VERSION = 6
+ABI_VERSION = 7
 STAGES = ("preprocess", "binning", "render_fwd", "render_bwd", "geom_bwd")
 
 
@@ -141,7 +141,7 @@ class AdamArgs(C.Structure):
 class Layout(C.Structure):
     _fields_ = [(n, C.c_size_t) for n in (
         "geom_rec", "geom_depth", "geom_rect", "geom_clamped", "img_final_T", "img_n_contrib",
-        "img_ranges", "img_tile_count", "bin_point_list", "bin_keys")]
+        "img_ranges", "img_tile_count", "bin_point_list", "bin_keys", "geom_acc")]
 
 
 _lib = None

@@ -36,6 +36,11 @@ WORKLOAD_TEXT = {
 }
 CAMS_PER_GPU = 8
 RING_RADIUS = 6.0          # SURVEY.md 8d: 64 cameras on a ring of radius 6 around the scene centre
+# torch's CPU elementwise kernels round the vectorised body of each thread's chunk and its scalar tail differently
+# (torch.sigmoid: a few of C3's 2 M opacities move by an ulp), so the scene's bits depend on how the tensors are split
+# among intra-op threads, i.e. on torch.get_num_threads().  Scenes are generated with this fixed split, so every machine
+# builds the same inputs; the reference outputs stored under tests/golden/ref were recorded with it.
+SCENE_THREADS = 16
 
 
 def camera_block(rank: int, world: int, n_cameras: int):
@@ -117,13 +122,20 @@ def build_workload(name, device, rank=0, world=1, cams_per_gpu=CAMS_PER_GPU, rin
         cams = [cam0] * len(block)     # free Gaussians are generated inside cam0's frustum
     wl = dict(name=name, P=P, W=W, H=H, D=D, kind=kind, cams=cams, ring_radius=ring_radius if kind == "frosting" else None)
     t = time.time()
+    threads = torch.get_num_threads()
+    torch.set_num_threads(SCENE_THREADS)
+    try:
+        if kind == "frosting":
+            params, mesh = scenes.frosting_layer(P, cam0, seed, n_faces_target=max(1000, P // 2), device="cpu")
+            attrs = scenes.frosting_attributes(params, mesh)
+        else:
+            attrs = scenes.random_gaussians(P, cam0, seed, device="cpu")
+    finally:
+        torch.set_num_threads(threads)
     if kind == "frosting":
-        params, mesh = scenes.frosting_layer(P, cam0, seed, n_faces_target=max(1000, P // 2), device="cpu")
-        attrs = scenes.frosting_attributes(params, mesh)
         wl["mesh"] = {k: v.to(device) for k, v in mesh.items()}
         wl["params"] = {k: v.to(device) for k, v in params.items()}
     else:
-        attrs = scenes.random_gaussians(P, cam0, seed, device="cpu")
         wl["mesh"] = None
     wl["attrs"] = {k: v.to(device).contiguous() for k, v in attrs.items()}
     g = torch.Generator().manual_seed(4321 + rank)

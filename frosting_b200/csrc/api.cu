@@ -281,6 +281,7 @@ int fb200_get_layout(int32_t P, int32_t W, int32_t H, int64_t capacity, fb200_la
     out->img_final_T = il.final_T; out->img_n_contrib = il.n_contrib; out->img_ranges = il.ranges;
     out->img_tile_count = il.tile_count;
     out->bin_point_list = bl.point_list; out->bin_keys = bl.keys;
+    out->geom_acc = gl.acc;
     return FB200_OK;
 }
 

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define FB200_ABI_VERSION 6
+#define FB200_ABI_VERSION 7
 
 #define FB200_OK 0
 #define FB200_EINVAL (-1)   /* bad argument (shape / null pointer / unsupported channel count) */
@@ -503,6 +503,10 @@ typedef struct fb200_layout {
     size_t img_tile_count; /* u32[T] */
     size_t bin_point_list; /* u32[capacity] sorted Gaussian index per instance */
     size_t bin_keys;       /* u64[capacity] (depth_bits<<32 | gaussian idx), sorted within each tile */
+    size_t geom_acc;       /* f32[12P] the blend backward's per-Gaussian accumulators, the per-Gaussian backward's input:
+                              {dmean2D.x, dmean2D.y, dconic.x, dconic.y}, {dconic.w, dopacity, dr, dg}, {db, e0, e1, e2}
+                              (e*: extra feature channels).  Valid after fb200_backward until the next forward or
+                              backward on the workspace */
 } fb200_layout;
 
 int fb200_get_layout(int32_t P, int32_t image_width, int32_t image_height, int64_t capacity,

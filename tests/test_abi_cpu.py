@@ -23,7 +23,7 @@ def test_every_declared_symbol_is_exported():
     for n in names:
         assert hasattr(L, n), f"{n} declared in the header but not exported"
     assert sorted(_lib.EXPORTED) == names, "frosting_b200/_lib.py:EXPORTED out of sync with the header"
-    assert L.fb200_abi_version() == _lib.ABI_VERSION == 6
+    assert L.fb200_abi_version() == _lib.ABI_VERSION == 7
 
 
 def test_workspace_size_queries_are_host_only_and_monotonic():
@@ -44,7 +44,7 @@ def test_layout_offsets_are_aligned_and_ordered():
     assert L.fb200_get_layout(1000, 256, 128, 5000, C.byref(lay)) == 0
     offs = [getattr(lay, n) for n, _ in _lib.Layout._fields_]
     assert all(o % 128 == 0 for o in offs)
-    assert lay.geom_rec < lay.geom_depth < lay.geom_rect < lay.geom_clamped
+    assert lay.geom_rec < lay.geom_depth < lay.geom_rect < lay.geom_clamped < lay.geom_acc
     assert lay.img_final_T < lay.img_n_contrib < lay.img_ranges < lay.img_tile_count
     assert lay.bin_point_list < lay.bin_keys
 
