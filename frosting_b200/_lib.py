@@ -28,6 +28,8 @@ EXPORTED = [
     "fb200_mesh_barycentrics", "fb200_texture_face_sh_colours", "fb200_texture_add_view", "fb200_texture_finish",
     "fb200_texture_struct_size",
     "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
+    "fb200_sugar_reg_workspace_bytes", "fb200_sugar_reg_forward", "fb200_sugar_reg_backward",
+    "fb200_sugar_reg_struct_size",
     "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
 ]
 NUM_STAGES = 5
@@ -118,6 +120,12 @@ class Texture(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_faces", "n_points", "square_size", "n_square_per_axis", "texture_size")] + \
                [(n, C.c_void_p) for n in ("d_cell_offsets", "d_cell_points", "d_sh_dc", "d_face_sh", "d_face_acc",
                                           "d_texel_acc", "d_face_winner", "d_texel_winner")]
+
+
+class SugarReg(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("P", "K", "N")] + [("sampling_scale_factor", C.c_float)] + \
+               [(n, C.c_void_p) for n in ("d_points", "d_scaling", "d_quaternions", "d_strengths", "d_knn_idx", "d_idx",
+                                          "d_eps", "d_workspace")]
 
 
 ADAM_MAX_GROUPS = 16
@@ -225,6 +233,13 @@ def lib():
     L.fb200_l1_dssim_backward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                           C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     L.fb200_l1_dssim_backward.restype = C.c_int
+    L.fb200_sugar_reg_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+    L.fb200_sugar_reg_workspace_bytes.restype = C.c_size_t
+    L.fb200_sugar_reg_forward.argtypes = [C.POINTER(SugarReg), C.c_int32, C.c_void_p, C.c_void_p]
+    L.fb200_sugar_reg_forward.restype = C.c_int
+    L.fb200_sugar_reg_backward.argtypes = [C.POINTER(SugarReg)] + [C.c_void_p] * 6
+    L.fb200_sugar_reg_backward.restype = C.c_int
+    L.fb200_sugar_reg_struct_size.restype = C.c_size_t
     L.fb200_adam_step.argtypes = [C.POINTER(AdamArgs), C.c_void_p]
     L.fb200_peer_alloc.argtypes = [C.c_size_t, C.POINTER(C.c_void_p)]
     L.fb200_peer_free.argtypes = [C.c_void_p]
@@ -257,6 +272,8 @@ def lib():
         raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_skin out of sync with include/frosting_b200.h")
     if L.fb200_texture_struct_size() != C.sizeof(Texture):
         raise RuntimeError("frosting_b200: ctypes mirror of fb200_texture out of sync with include/frosting_b200.h")
+    if L.fb200_sugar_reg_struct_size() != C.sizeof(SugarReg):
+        raise RuntimeError("frosting_b200: ctypes mirror of fb200_sugar_reg out of sync with include/frosting_b200.h")
     _lib = L
     return L
 

@@ -706,6 +706,48 @@ int fb200_l1_dssim_backward(const float* d_pred, const float* d_gt, const float*
                                      static_cast<cudaStream_t>(stream)), "l1_dssim_backward");
 }
 
+size_t fb200_sugar_reg_struct_size(void) { return sizeof(fb200_sugar_reg); }
+
+size_t fb200_sugar_reg_workspace_bytes(int32_t P, int32_t K, int32_t N, int32_t with_grad) {
+    return (P >= 0 && K >= 1 && K <= 32 && N >= 0) ? sugar_reg_workspace_bytes(P, K, N, with_grad != 0) : 0;
+}
+
+static int check_sugar_reg(const fb200_sugar_reg* r) {
+    if (!r) return fail(FB200_EINVAL, "sugar_reg: null struct%s");
+    if (r->P < 0 || r->N < 0 || (r->N > 0 && r->P == 0))
+        return fail(FB200_EINVAL, "sugar_reg: bad extents (P >= 0, N >= 0, P > 0 when N > 0)%s");
+    if (r->K < 1 || r->K > 32) return fail(FB200_EINVAL, "sugar_reg: K must be within [1, 32]%s");
+    if (!r->d_workspace) return fail(FB200_EINVAL, "sugar_reg: missing workspace%s");
+    if (r->P > 0 && (!r->d_points || !r->d_scaling || !r->d_quaternions || !r->d_strengths || !r->d_knn_idx))
+        return fail(FB200_EINVAL, "sugar_reg: missing Gaussian pointer%s");
+    if (r->N > 0 && (!r->d_idx || !r->d_eps)) return fail(FB200_EINVAL, "sugar_reg: missing sample pointer%s");
+    if (misaligned(r->d_quaternions, 16) || misaligned(r->d_workspace, 16))
+        return fail(FB200_EINVAL, "sugar_reg: quaternions and workspace must be 16-byte aligned%s");
+    return FB200_OK;
+}
+
+int fb200_sugar_reg_forward(const fb200_sugar_reg* r, int32_t with_grad, float* d_terms, void* stream) {
+    int rc = check_sugar_reg(r);
+    if (rc != FB200_OK) return rc;
+    if (!d_terms) return fail(FB200_EINVAL, "sugar_reg_forward: missing terms output%s");
+    return check(launch_sugar_reg_fwd(*r, with_grad != 0, d_terms, static_cast<cudaStream_t>(stream)),
+                 "sugar_reg_forward");
+}
+
+int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms, float* d_dpoints, float* d_dscaling,
+                             float* d_dquaternions, float* d_dstrengths, void* stream) {
+    int rc = check_sugar_reg(r);
+    if (rc != FB200_OK) return rc;
+    if (r->P == 0) return FB200_OK;
+    if (!d_dL_dterms || !d_dpoints || !d_dscaling || !d_dquaternions || !d_dstrengths)
+        return fail(FB200_EINVAL, "sugar_reg_backward: missing gradient pointer%s");
+    if (misaligned(d_dquaternions, 16))
+        return fail(FB200_EINVAL, "sugar_reg_backward: dL/dquaternions must be 16-byte aligned%s");
+    return check(launch_sugar_reg_bwd(*r, d_dL_dterms, d_dpoints, d_dscaling, d_dquaternions, d_dstrengths,
+                                      static_cast<cudaStream_t>(stream)),
+                 "sugar_reg_backward");
+}
+
 int fb200_adam_step(const fb200_adam_args* a, void* stream) {
     if (!a) return fail(FB200_EINVAL, "adam_step: null args%s");
     if (a->world < 1 || a->world > FB200_MAX_PEERS || a->rank < 0 || a->rank >= a->world)

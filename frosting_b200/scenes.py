@@ -307,6 +307,22 @@ def quaternion_to_matrix(q):
     return m.reshape(q.shape[:-1] + (3, 3))
 
 
+def quaternion_apply(q, v):
+    """q * (0, v) * quaternion_invert(q), vector part: pytorch3d's quaternion_apply (no normalisation of q, so a
+    non-unit q also scales by |q|^2)."""
+    p = quaternion_raw_multiply(quaternion_raw_multiply(q, torch.cat([v.new_zeros(v.shape[:-1] + (1,)), v], -1)),
+                                quaternion_invert(q))
+    return p[..., 1:]
+
+
+def quaternion_raw_multiply(a, b):
+    """Hamilton product of (w, x, y, z) quaternions, without standardisation."""
+    aw, ax, ay, az = a.unbind(-1)
+    bw, bx, by, bz = b.unbind(-1)
+    return torch.stack([aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+                        aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw], -1)
+
+
 def matrix_to_quaternion(m):
     """The candidate quaternion of the largest |q_c| (first on ties), over 2 max(|q_c|, 0.1); standardised."""
     m00, m01, m02, m10, m11, m12, m20, m21, m22 = m.reshape(m.shape[:-2] + (9,)).unbind(-1)
@@ -723,3 +739,45 @@ def bake_texture_torch(n_faces, cells, sh_dc, square_size, images, pix_to_faces,
     face_colors[~visited] = sh_colors[~visited]
     texture_img[~filled] = face_colors[uv_to_faces[~filled]]
     return verts_uv, faces_uv, texture_img.flip(0)
+
+
+# ---- SuGaR coarse-stage scenes (SURVEY.md row a23): the SDF regulariser's inputs ----
+
+def sugar_scene(P, seed, K=16, straggler_frac=0.1, device="cpu"):
+    """A SuGaR-like coarse scene of P Gaussians as the trainer holds them after activation: flat Gaussians on a bumpy
+    sphere (radius 2 around (0, 0, 6), in front of `make_camera`'s default camera), the thin axis along the surface normal
+    and at a random index, plus `straggler_frac` volumetric Gaussians scattered around it.  Returns points [P,3],
+    scaling [P,3], unit quaternions [P,4], strengths [P,1] and the K-nearest-neighbour table knn_idx [P,K] (int64,
+    scipy cKDTree, self first, as pytorch3d knn_points on distinct points)."""
+    from scipy.spatial import cKDTree
+    g = torch.Generator().manual_seed(seed)
+    n_flat = P - int(straggler_frac * P)
+    d = torch.nn.functional.normalize(torch.randn(P, 3, generator=g), dim=-1)
+    bump = 1.0 + 0.08 * torch.sin(5 * d[:, 0]) * torch.cos(4 * d[:, 1])
+    spacing = math.sqrt(4 * math.pi * 4.0 / max(P, 1))
+    centre = torch.tensor([0.0, 0.0, 6.0])
+    points = centre + 2.0 * bump[:, None] * d
+    scaling = spacing * torch.exp(0.3 * torch.randn(P, 3, generator=g))
+    # the normal axis: a random column of a random frame whose column c is the sphere's normal
+    c = torch.randint(0, 3, (P,), generator=g)
+    t1 = torch.nn.functional.normalize(torch.linalg.cross(d, torch.randn(P, 3, generator=g), dim=-1), dim=-1)
+    t2 = torch.linalg.cross(d, t1, dim=-1)
+    R = torch.zeros(P, 3, 3)
+    for k in range(3):
+        pick = c == k
+        R[pick, :, k] = d[pick]
+        R[pick, :, (k + 1) % 3] = t1[pick]
+        R[pick, :, (k + 2) % 3] = t2[pick]
+    thin = spacing * 0.02 * torch.exp(0.5 * torch.randn(P, generator=g))
+    scaling[torch.arange(P), c] = thin
+    q = matrix_to_quaternion(R)
+    # stragglers: volumetric, anywhere within 0.3 of the surface, random orientation
+    s = slice(n_flat, P)
+    points[s] += 0.3 * torch.randn(P - n_flat, 3, generator=g)
+    scaling[s] = 3 * spacing * torch.exp(0.3 * torch.randn(P - n_flat, 3, generator=g))
+    q[s] = torch.randn(P - n_flat, 4, generator=g)
+    q = torch.nn.functional.normalize(q, dim=-1)
+    strengths = torch.sigmoid(2.0 * torch.randn(P, 1, generator=g))
+    knn = torch.from_numpy(cKDTree(points.double().numpy()).query(points.double().numpy(), k=K)[1]).long().reshape(P, K)
+    to =lambda t: t.contiguous().to(device)
+    return dict(points=to(points), scaling=to(scaling), quaternions=to(q), strengths=to(strengths), knn_idx=to(knn))

@@ -433,6 +433,46 @@ int fb200_l1_dssim_forward(const float* d_pred, const float* d_gt, int32_t C, in
 int fb200_l1_dssim_backward(const float* d_pred, const float* d_gt, const float* d_maps, int32_t C, int32_t H,
                             int32_t W, float lambda, const float* d_dL_dloss, float* d_dpred, void* stream);
 
+/* SuGaR's SDF regulariser of the coarse stage (SURVEY.md row a23; frosting_trainers/coarse_density_and_dn_consistency.py
+ * :745-833 with frosting_scene/sugar_model.py get_field_values, get_beta 'average', get_smallest_axis; density-mode
+ * estimation, gradient through the normals only).  For sample n with owner i = d_idx[n] and neighbours
+ * j = d_knn_idx[i,k], k < K:
+ *   x = mu_i + q_i ((f s_i) * eps_n) q_i^-1 (pytorch3d quaternion_apply: the conjugate as inverse);
+ *   A_j = quaternion_to_matrix(q_j) with column c scaled by 1 / clamp(s_jc, 1e-8);
+ *   o_k = sigma_j exp(-clamp(|A_j^T (x - mu_j)|^2, 0, 1e8) / 2), d = sum_k o_k, beta = mean_k min s_j;
+ *   nrm = the column of R(q) at the first minimal axis of s; sdf = (x - mu_i) . nrm_i, t = exp(-sdf^2 / (2 beta^2));
+ *   m_k = nrm_j sign(nrm_j . nrm_i); w_k = o_k |(x - mu_j) . m_k| / clamp(min s_j, 1e-6)^2 (no gradient);
+ *   terms[0] = mean_n |d - t|;  terms[1] = mean_n |nrm_i - sum_k w_k m_k / clamp(sum_k w_k, 1e-6)|^2.
+ * The workspace (fb200_sugar_reg_workspace_bytes, 16-byte aligned) holds an 80-byte record per Gaussian and 8 bytes
+ * per block of samples, and for with_grad a 128-byte gradient accumulator per Gaussian (replicated to fill 32 MiB when
+ * P < 2^18); nothing of size N x K.  A forward without gradient needs only the with_grad = 0 size.
+ * fb200_sugar_reg_forward writes d_terms [2]; with `with_grad` it also differentiates both terms at unit upstream
+ * into the workspace, and fb200_sugar_reg_backward then writes the dense gradients of terms[0] * d_dL_dterms[0] +
+ * terms[1] * d_dL_dterms[1] (a device [2]) with respect to the four inputs, reading the same struct.  A sample whose
+ * owner d_idx[n] lies outside [0, P) is skipped and makes both terms NaN (checked on the device, no synchronisation);
+ * d_knn_idx is not checked and must lie in [0, P). */
+typedef struct fb200_sugar_reg {
+    int32_t P;                      /* Gaussians */
+    int32_t K;                      /* neighbours per Gaussian, 1..32 */
+    int32_t N;                      /* samples; N > 0 needs P > 0 */
+    float sampling_scale_factor;    /* f (1.5 in the trainers) */
+    const float* d_points;          /* [P,3] */
+    const float* d_scaling;         /* [P,3] activated scales */
+    const float* d_quaternions;     /* [P,4] (w, x, y, z), 16-byte aligned */
+    const float* d_strengths;       /* [P] activated opacities */
+    const int32_t* d_knn_idx;       /* [P,K] */
+    const int64_t* d_idx;           /* [N] owner Gaussian of each sample */
+    const float* d_eps;             /* [N,3] standard normal draws */
+    void* d_workspace;              /* fb200_sugar_reg_workspace_bytes(P, K, N, with_grad) bytes */
+} fb200_sugar_reg;
+size_t fb200_sugar_reg_workspace_bytes(int32_t P, int32_t K, int32_t N, int32_t with_grad);
+int fb200_sugar_reg_forward(const fb200_sugar_reg* r, int32_t with_grad, float* d_terms, void* stream);
+/* d_dquaternions 16-byte aligned.  Needs a preceding fb200_sugar_reg_forward with_grad on the same workspace. */
+int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms, float* d_dpoints, float* d_dscaling,
+                             float* d_dquaternions, float* d_dstrengths, void* stream);
+/* sizeof(fb200_sugar_reg), for binding mirrors */
+size_t fb200_sugar_reg_struct_size(void);
+
 /* Data-parallel gradient reduction fused with the Adam update (SURVEY.md row f3).  Replaces "all-reduce every
  * .grad, then torch.optim.Adam(l, lr=0.0, eps=1e-15).step()" (frosting_scene/frosting_optimizer.py:101,116-118) for
  * camera-sharded training.  All learnable tensors of a rank live in ONE flat fp32 parameter slab and their gradients
