@@ -14,26 +14,8 @@ LIB_PATH = os.path.join(_HERE, "libfrosting_b200.so")
 FB200_STATUS_WORDS = 8
 ST_NUM_RENDERED, ST_OVERFLOW, ST_MAX_TILE, ST_NUM_VISIBLE = 0, 1, 2, 3
 TILE = 16
-
-# every symbol include/frosting_b200.h declares
-EXPORTED = [
-    "fb200_abi_version", "fb200_abi_struct_sizes", "fb200_last_error", "fb200_geom_bytes", "fb200_image_bytes",
-    "fb200_binning_bytes", "fb200_forward", "fb200_forward_geometry", "fb200_forward_raster", "fb200_backward", "fb200_mark_visible",
-    "fb200_mesh_visibility", "fb200_gaussian_mask_from_faces", "fb200_get_layout",
-    "fb200_profile_enable", "fb200_profile_read", "fb200_kernel_launches",
-    "fb200_frosting_attributes", "fb200_frosting_attributes_backward",
-    "fb200_frosting_edit_shell", "fb200_frosting_edit_attributes", "fb200_frosting_edit_struct_size",
-    "fb200_frosting_edit_complex_capture", "fb200_frosting_edit_attributes_complex",
-    "fb200_frosting_skin_pose", "fb200_frosting_skin_struct_size",
-    "fb200_mesh_barycentrics", "fb200_texture_face_sh_colours", "fb200_texture_add_view", "fb200_texture_finish",
-    "fb200_texture_struct_size",
-    "fb200_loss_partials", "fb200_l1_dssim_forward", "fb200_l1_dssim_backward",
-    "fb200_sugar_reg_workspace_bytes", "fb200_sugar_reg_forward", "fb200_sugar_reg_backward",
-    "fb200_sugar_reg_struct_size",
-    "fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open", "fb200_peer_close",
-]
 NUM_STAGES = 5
-ABI_VERSION = 7
+ABI_VERSION = 8
 STAGES = ("preprocess", "binning", "render_fwd", "render_bwd", "geom_bwd")
 
 
@@ -152,6 +134,65 @@ class Layout(C.Structure):
         "img_ranges", "img_tile_count", "bin_point_list", "bin_keys", "geom_acc")]
 
 
+# (C struct, ctypes mirror) in the order fb200_abi_struct_sizes reports them (FB200_ABI_STRUCTS)
+ABI_STRUCTS = (
+    ("fb200_params", Params), ("fb200_inputs", Inputs), ("fb200_workspace", Workspace), ("fb200_grads", Grads),
+    ("fb200_extra", Extra), ("fb200_frosting_params", FrostingParams), ("fb200_frosting_grads", FrostingGrads),
+    ("fb200_adam_args", AdamArgs), ("fb200_layout", Layout), ("fb200_frosting_edit", FrostingEdit),
+    ("fb200_frosting_skin", FrostingSkin), ("fb200_texture", Texture), ("fb200_sugar_reg", SugarReg),
+)
+
+_i32, _i64, _f32, _vp, _int, _size = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_int, C.c_size_t
+_frame = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace)]
+
+# name -> (restype, argtypes) of every function include/frosting_b200.h declares; tests/test_abi_cpu.py checks each
+# against its prototype
+SIGNATURES = {
+    "fb200_geom_bytes": (_size, [_i32]),
+    "fb200_image_bytes": (_size, [_i32, _i32]),
+    "fb200_binning_bytes": (_size, [_i64]),
+    "fb200_forward": (_int, _frame + [_vp, _vp, _vp]),
+    "fb200_forward_geometry": (_int, _frame + [_vp, _vp]),
+    "fb200_forward_raster": (_int, _frame + [_vp, _vp, _vp]),
+    "fb200_backward": (_int, _frame + [_vp, _vp, C.POINTER(Grads), _vp]),
+    "fb200_mark_visible": (_int, [_i32, _vp, _vp, _vp, _vp, _vp]),
+    "fb200_mesh_visibility": (_int, [_i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _vp, _vp]),
+    "fb200_gaussian_mask_from_faces": (_int, [_i32, _vp, _i32, _vp, _i32, _vp, _vp]),
+    "fb200_frosting_attributes": (_int, [C.POINTER(FrostingParams)] + [_vp] * 6),
+    "fb200_frosting_attributes_backward": (_int, [C.POINTER(FrostingParams)] + [_vp] * 5 +
+                                           [C.POINTER(FrostingGrads), _vp]),
+    "fb200_frosting_edit_shell": (_int, [C.POINTER(FrostingEdit), _vp]),
+    "fb200_frosting_edit_attributes": (_int, [C.POINTER(FrostingEdit), C.POINTER(FrostingParams), _i32] + [_vp] * 8),
+    "fb200_frosting_edit_complex_capture": (_int, [C.POINTER(FrostingEdit), C.POINTER(FrostingParams)] + [_vp] * 4),
+    "fb200_frosting_edit_attributes_complex": (_int, [C.POINTER(FrostingEdit), C.POINTER(FrostingParams), _i32] +
+                                               [_vp] * 10),
+    "fb200_frosting_skin_pose": (_int, [C.POINTER(FrostingSkin), _i32, _vp, _vp]),
+    "fb200_mesh_barycentrics": (_int, [_i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
+    "fb200_texture_face_sh_colours": (_int, [C.POINTER(Texture), _vp]),
+    "fb200_texture_add_view": (_int, [C.POINTER(Texture), _vp, _vp, _vp, _i32, _i32, _vp]),
+    "fb200_texture_finish": (_int, [C.POINTER(Texture), _vp, _vp]),
+    "fb200_loss_partials": (_size, [_i32, _i32, _i32]),
+    "fb200_l1_dssim_forward": (_int, [_vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp]),
+    "fb200_l1_dssim_backward": (_int, [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp]),
+    "fb200_sugar_reg_workspace_bytes": (_size, [_i32, _i32, _i32, _i32]),
+    "fb200_sugar_reg_forward": (_int, [C.POINTER(SugarReg), _i32, _vp, _vp]),
+    "fb200_sugar_reg_backward": (_int, [C.POINTER(SugarReg)] + [_vp] * 6),
+    "fb200_adam_step": (_int, [C.POINTER(AdamArgs), _vp]),
+    "fb200_peer_alloc": (_int, [_size, C.POINTER(_vp)]),
+    "fb200_peer_free": (_int, [_vp]),
+    "fb200_peer_export": (_int, [_vp, C.c_char_p]),
+    "fb200_peer_open": (_int, [C.c_char_p, C.POINTER(_vp)]),
+    "fb200_peer_close": (_int, [_vp]),
+    "fb200_get_layout": (_int, [_i32, _i32, _i32, _i64, C.POINTER(Layout)]),
+    "fb200_profile_enable": (_int, [_i32]),
+    "fb200_profile_read": (_int, [C.POINTER(_f32)]),
+    "fb200_kernel_launches": (_i64, []),
+    "fb200_last_error": (C.c_char_p, []),
+    "fb200_abi_version": (_int, []),
+    "fb200_abi_struct_sizes": (_int, [C.POINTER(_size)]),
+}
+EXPORTED = list(SIGNATURES)
+
 _lib = None
 
 
@@ -173,107 +214,17 @@ def lib():
                 f"frosting_b200: CUDA library {LIB_PATH} is missing and could not be built ({ex}). "
                 "Run `python -m frosting_b200.build`. There is no CPU fallback.") from ex
     L = C.CDLL(LIB_PATH)
-    L.fb200_abi_version.restype = C.c_int
-    L.fb200_last_error.restype = C.c_char_p
-    for n in ("fb200_geom_bytes", "fb200_image_bytes", "fb200_binning_bytes"):
-        getattr(L, n).restype = C.c_size_t
-    L.fb200_geom_bytes.argtypes = [C.c_int32]
-    L.fb200_image_bytes.argtypes = [C.c_int32, C.c_int32]
-    L.fb200_binning_bytes.argtypes = [C.c_int64]
-    L.fb200_forward.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace),
-                                C.c_void_p, C.c_void_p, C.c_void_p]
-    L.fb200_forward_geometry.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace),
-                                         C.c_void_p, C.c_void_p]
-    L.fb200_forward_raster.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace),
-                                       C.c_void_p, C.c_void_p, C.c_void_p]
-    L.fb200_backward.argtypes = [C.POINTER(Params), C.POINTER(Inputs), C.POINTER(Workspace),
-                                 C.c_void_p, C.c_void_p, C.POINTER(Grads), C.c_void_p]
-    L.fb200_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.fb200_mesh_visibility.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_int32, C.c_void_p, C.c_void_p]
-    L.fb200_gaussian_mask_from_faces.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
-                                                 C.c_void_p, C.c_void_p]
-    L.fb200_get_layout.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.POINTER(Layout)]
-    L.fb200_frosting_attributes.argtypes = [C.POINTER(FrostingParams)] + [C.c_void_p] * 6
-    L.fb200_frosting_attributes.restype = C.c_int
-    L.fb200_frosting_attributes_backward.argtypes = [C.POINTER(FrostingParams)] + [C.c_void_p] * 5 + \
-        [C.POINTER(FrostingGrads), C.c_void_p]
-    L.fb200_frosting_attributes_backward.restype = C.c_int
-    L.fb200_frosting_edit_shell.argtypes = [C.POINTER(FrostingEdit), C.c_void_p]
-    L.fb200_frosting_edit_shell.restype = C.c_int
-    L.fb200_frosting_edit_attributes.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams), C.c_int32] + \
-        [C.c_void_p] * 8
-    L.fb200_frosting_edit_attributes.restype = C.c_int
-    L.fb200_frosting_edit_struct_size.restype = C.c_size_t
-    L.fb200_frosting_edit_complex_capture.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams)] + \
-        [C.c_void_p] * 4
-    L.fb200_frosting_edit_complex_capture.restype = C.c_int
-    L.fb200_frosting_edit_attributes_complex.argtypes = [C.POINTER(FrostingEdit), C.POINTER(FrostingParams),
-                                                         C.c_int32] + [C.c_void_p] * 10
-    L.fb200_frosting_edit_attributes_complex.restype = C.c_int
-    L.fb200_frosting_skin_pose.argtypes = [C.POINTER(FrostingSkin), C.c_int32, C.c_void_p, C.c_void_p]
-    L.fb200_frosting_skin_pose.restype = C.c_int
-    L.fb200_frosting_skin_struct_size.restype = C.c_size_t
-    L.fb200_mesh_barycentrics.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                                          C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.fb200_texture_face_sh_colours.argtypes = [C.POINTER(Texture), C.c_void_p]
-    L.fb200_texture_add_view.argtypes = [C.POINTER(Texture), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
-                                         C.c_void_p]
-    L.fb200_texture_finish.argtypes = [C.POINTER(Texture), C.c_void_p, C.c_void_p]
-    for n in ("fb200_mesh_barycentrics", "fb200_texture_face_sh_colours", "fb200_texture_add_view",
-              "fb200_texture_finish"):
-        getattr(L, n).restype = C.c_int
-    L.fb200_texture_struct_size.restype = C.c_size_t
-    L.fb200_loss_partials.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    L.fb200_loss_partials.restype = C.c_size_t
-    L.fb200_l1_dssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
-                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.fb200_l1_dssim_forward.restype = C.c_int
-    L.fb200_l1_dssim_backward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                          C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.fb200_l1_dssim_backward.restype = C.c_int
-    L.fb200_sugar_reg_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
-    L.fb200_sugar_reg_workspace_bytes.restype = C.c_size_t
-    L.fb200_sugar_reg_forward.argtypes = [C.POINTER(SugarReg), C.c_int32, C.c_void_p, C.c_void_p]
-    L.fb200_sugar_reg_forward.restype = C.c_int
-    L.fb200_sugar_reg_backward.argtypes = [C.POINTER(SugarReg)] + [C.c_void_p] * 6
-    L.fb200_sugar_reg_backward.restype = C.c_int
-    L.fb200_sugar_reg_struct_size.restype = C.c_size_t
-    L.fb200_adam_step.argtypes = [C.POINTER(AdamArgs), C.c_void_p]
-    L.fb200_peer_alloc.argtypes = [C.c_size_t, C.POINTER(C.c_void_p)]
-    L.fb200_peer_free.argtypes = [C.c_void_p]
-    L.fb200_peer_export.argtypes = [C.c_void_p, C.c_char_p]
-    L.fb200_peer_open.argtypes = [C.c_char_p, C.POINTER(C.c_void_p)]
-    L.fb200_peer_close.argtypes = [C.c_void_p]
-    for n in ("fb200_adam_step", "fb200_peer_alloc", "fb200_peer_free", "fb200_peer_export", "fb200_peer_open",
-              "fb200_peer_close"):
-        getattr(L, n).restype = C.c_int
-    L.fb200_profile_enable.argtypes = [C.c_int32]
-    L.fb200_profile_enable.restype = C.c_int
-    L.fb200_profile_read.argtypes = [C.POINTER(C.c_float)]
-    L.fb200_profile_read.restype = C.c_int
-    L.fb200_kernel_launches.restype = C.c_int64
-    for n in ("fb200_forward", "fb200_forward_geometry", "fb200_forward_raster", "fb200_backward", "fb200_mark_visible", "fb200_mesh_visibility",
-              "fb200_gaussian_mask_from_faces", "fb200_get_layout"):
-        getattr(L, n).restype = C.c_int
+    # before anything else: the exported names and the struct count depend on the version (an int(void) function,
+    # callable with ctypes' default signature)
     if L.fb200_abi_version() != ABI_VERSION:
         raise RuntimeError("frosting_b200: ABI version mismatch between header and library")
-    mirrors = (Params, Inputs, Workspace, Grads, Extra, FrostingParams, FrostingGrads, AdamArgs, Layout)
-    sizes = (C.c_size_t * len(mirrors))()
-    L.fb200_abi_struct_sizes.argtypes = [C.POINTER(C.c_size_t)]
-    L.fb200_abi_struct_sizes.restype = C.c_int
-    if L.fb200_abi_struct_sizes(sizes) != 0 or [int(x) for x in sizes] != [C.sizeof(m) for m in mirrors]:
-        raise RuntimeError("frosting_b200: ctypes struct mirrors out of sync with include/frosting_b200.h: "
-                           f"{[int(x) for x in sizes]} vs {[C.sizeof(m) for m in mirrors]}")
-    if L.fb200_frosting_edit_struct_size() != C.sizeof(FrostingEdit):
-        raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_edit out of sync with include/frosting_b200.h")
-    if L.fb200_frosting_skin_struct_size() != C.sizeof(FrostingSkin):
-        raise RuntimeError("frosting_b200: ctypes mirror of fb200_frosting_skin out of sync with include/frosting_b200.h")
-    if L.fb200_texture_struct_size() != C.sizeof(Texture):
-        raise RuntimeError("frosting_b200: ctypes mirror of fb200_texture out of sync with include/frosting_b200.h")
-    if L.fb200_sugar_reg_struct_size() != C.sizeof(SugarReg):
-        raise RuntimeError("frosting_b200: ctypes mirror of fb200_sugar_reg out of sync with include/frosting_b200.h")
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    sizes = (C.c_size_t * len(ABI_STRUCTS))()
+    if L.fb200_abi_struct_sizes(sizes) != 0 or list(sizes) != [C.sizeof(m) for _, m in ABI_STRUCTS]:
+        raise RuntimeError("frosting_b200: ctypes struct mirrors out of sync with include/frosting_b200.h: " +
+                           ", ".join(f"{n} {s} vs {C.sizeof(m)}" for (n, m), s in zip(ABI_STRUCTS, sizes)))
     _lib = L
     return L
 

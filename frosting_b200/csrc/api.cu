@@ -17,8 +17,8 @@ namespace {
 
 thread_local char g_err[512] = "";
 
-int fail(int code, const char* fmt, const char* detail = "") {
-    snprintf(g_err, sizeof(g_err), fmt, detail);
+int fail(int code, const char* msg) {
+    snprintf(g_err, sizeof(g_err), "%s", msg);
     return code;
 }
 
@@ -42,23 +42,23 @@ bool misaligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintp
 // (header: fb200_frosting_params): bary logits as float2, quats as float4, and the sh_rest rows moved as float4 blocks of
 // a warp's 32 rows (frosting_attr.cu)
 int check_frosting(const fb200_frosting_params* fp) {
-    if (!fp) return fail(FB200_EINVAL, "frosting_attributes: null params%s");
+    if (!fp) return fail(FB200_EINVAL, "frosting_attributes: null params");
     if (fp->P < 0 || fp->sh_rest < 0 || fp->n_verts < 0 || fp->n_faces < 0)
-        return fail(FB200_EINVAL, "frosting_attributes: bad extents%s");
+        return fail(FB200_EINVAL, "frosting_attributes: bad extents");
     if (fp->P > 0 && (!fp->d_bary_logits || !fp->d_cells || !fp->d_faces || !fp->d_inner_verts || !fp->d_outer_verts ||
                       !fp->d_opacity_logits || !fp->d_log_scales || !fp->d_quats || !fp->d_sh_dc ||
                       (fp->sh_rest > 0 && !fp->d_sh_rest)))
-        return fail(FB200_EINVAL, "frosting_attributes: missing parameter pointer%s");
+        return fail(FB200_EINVAL, "frosting_attributes: missing parameter pointer");
     if (fp->P > 0 && (misaligned(fp->d_bary_logits, 8) || misaligned(fp->d_quats, 16) ||
                       (fp->sh_rest > 0 && misaligned(fp->d_sh_rest, 16))))
-        return fail(FB200_EINVAL, "frosting_attributes: bary logits must be 8-byte, quats and sh_rest 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting_attributes: bary logits must be 8-byte, quats and sh_rest 16-byte aligned");
     // background Gaussians
-    if (fp->n_bg < 0) return fail(FB200_EINVAL, "frosting background: n_bg must be >= 0%s");
+    if (fp->n_bg < 0) return fail(FB200_EINVAL, "frosting background: n_bg must be >= 0");
     if (fp->n_bg > 0 && (!fp->d_bg_points || !fp->d_bg_opacity_logits || !fp->d_bg_log_scales || !fp->d_bg_quats ||
                          !fp->d_bg_sh_dc || (fp->sh_rest > 0 && !fp->d_bg_sh_rest)))
-        return fail(FB200_EINVAL, "frosting background: missing parameter pointer%s");
+        return fail(FB200_EINVAL, "frosting background: missing parameter pointer");
     if (fp->n_bg > 0 && misaligned(fp->d_bg_quats, 16))
-        return fail(FB200_EINVAL, "frosting background: quats must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting background: quats must be 16-byte aligned");
     return FB200_OK;
 }
 
@@ -67,24 +67,24 @@ int check_frosting(const fb200_frosting_params* fp) {
 // attribute backward zero-fills a warp's rows with float4 stores and stores quats as float4).  Background rows: given
 // exactly when there are background Gaussians, quats stored as float4.
 int check_frosting_grads(const fb200_frosting_params* fp, const fb200_frosting_grads* g) {
-    if (!g) return fail(FB200_EINVAL, "frosting gradients: null gradient block%s");
+    if (!g) return fail(FB200_EINVAL, "frosting gradients: null gradient block");
     if (fp->P > 0 && (!g->d_bary_logits || !g->d_opacity_logits || !g->d_log_scales || !g->d_quats || !g->d_sh_dc ||
                       (fp->sh_rest > 0 && !g->d_sh_rest) || ((g->d_inner_verts == nullptr) != (g->d_outer_verts == nullptr))))
-        return fail(FB200_EINVAL, "frosting gradients: parameter-gradient pointers missing%s");
+        return fail(FB200_EINVAL, "frosting gradients: parameter-gradient pointers missing");
     if (fp->P > 0 && (misaligned(g->d_bary_logits, 16) || misaligned(g->d_opacity_logits, 16) ||
                       misaligned(g->d_log_scales, 16) || misaligned(g->d_quats, 16) || misaligned(g->d_sh_dc, 16) ||
                       (fp->sh_rest > 0 && misaligned(g->d_sh_rest, 16))))
-        return fail(FB200_EINVAL, "frosting gradients: the mesh parameter gradients must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting gradients: the mesh parameter gradients must be 16-byte aligned");
     const bool any = g->d_bg_points || g->d_bg_opacity_logits || g->d_bg_log_scales || g->d_bg_quats || g->d_bg_sh_dc ||
                      g->d_bg_sh_rest;
     if (any != (fp->n_bg > 0))
         return fail(FB200_EINVAL, "frosting background: give background gradients exactly when there are background "
-                                  "Gaussians (n_bg > 0)%s");
+                                  "Gaussians (n_bg > 0)");
     if (fp->n_bg > 0 && (!g->d_bg_points || !g->d_bg_opacity_logits || !g->d_bg_log_scales || !g->d_bg_quats ||
                          !g->d_bg_sh_dc || (fp->sh_rest > 0 && !g->d_bg_sh_rest)))
-        return fail(FB200_EINVAL, "frosting background: gradient pointers missing%s");
+        return fail(FB200_EINVAL, "frosting background: gradient pointers missing");
     if (fp->n_bg > 0 && misaligned(g->d_bg_quats, 16))
-        return fail(FB200_EINVAL, "frosting background: dL/dquats must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting background: dL/dquats must be 16-byte aligned");
     return FB200_OK;
 }
 
@@ -95,13 +95,13 @@ int validate_frosting(const fb200_params* prm, const fb200_inputs* in) {
     if (rc != FB200_OK) return rc;
     if (in->d_means3D || in->d_shs || in->d_colors_precomp || in->d_opacities || in->d_scales || in->d_rotations ||
         in->d_cov3D_precomp || in->d_visibility || in->d_point_cells || in->d_face_visible)
-        return fail(FB200_EINVAL, "frosting mode: the attribute / mask pointers of fb200_inputs must be NULL%s");
+        return fail(FB200_EINVAL, "frosting mode: the attribute / mask pointers of fb200_inputs must be NULL");
     if ((int64_t)fp->P + fp->n_bg != prm->P || prm->sh_coeffs != fp->sh_rest + 1 || fp->sh_rest > 15)
         return fail(FB200_EINVAL, "frosting mode: P / sh_coeffs do not match the parameter block (P = frosting->P + "
-                                  "frosting->n_bg, sh_rest <= 15)%s");
+                                  "frosting->n_bg, sh_rest <= 15)");
     if (prm->sh_degree < 0 || prm->sh_degree > 3 || (prm->sh_degree + 1) * (prm->sh_degree + 1) > prm->sh_coeffs)
-        return fail(FB200_EINVAL, "sh_degree / sh_coeffs inconsistent%s");
-    if (prm->extra) return fail(FB200_EINVAL, "frosting mode: extra feature channels are not supported%s");
+        return fail(FB200_EINVAL, "sh_degree / sh_coeffs inconsistent");
+    if (prm->extra) return fail(FB200_EINVAL, "frosting mode: extra feature channels are not supported");
     return FB200_OK;
 }
 
@@ -116,52 +116,51 @@ fb200_inputs frosting_inputs(const fb200_inputs* in) {
 }
 
 int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws) {
-    if (!prm || !in || !ws) return fail(FB200_EINVAL, "null argument struct%s");
+    if (!prm || !in || !ws) return fail(FB200_EINVAL, "null argument struct");
     if (prm->P < 0 || prm->image_width <= 0 || prm->image_height <= 0)
-        return fail(FB200_EINVAL, "bad extents (P >= 0, image dims > 0 required)%s");
+        return fail(FB200_EINVAL, "bad extents (P >= 0, image dims > 0 required)");
     if (prm->image_width > 65535 * FB200_TILE || prm->image_height > 65535 * FB200_TILE)
-        return fail(FB200_EINVAL, "image too large for 16-bit tile coordinates%s");
+        return fail(FB200_EINVAL, "image too large for 16-bit tile coordinates");
     if (prm->debug & ~3)
-        return fail(FB200_EINVAL, "debug: only bits 0 (synchronise) and 1 (no sub-tile culling) are defined%s");
+        return fail(FB200_EINVAL, "debug: only bits 0 (synchronise) and 1 (no sub-tile culling) are defined");
     if (in->frosting) {
         int rc = validate_frosting(prm, in);
         if (rc != FB200_OK) return rc;
     } else if (prm->P > 0) {
-        if (!in->d_means3D || !in->d_opacities) return fail(FB200_EINVAL, "means3D / opacities missing%s");
+        if (!in->d_means3D || !in->d_opacities) return fail(FB200_EINVAL, "means3D / opacities missing");
         const bool has_sh = in->d_shs != nullptr, has_col = in->d_colors_precomp != nullptr;
         if (has_sh == has_col)
-            return fail(FB200_EINVAL, "Please provide excatly one of either SHs or precomputed colors!%s");
+            return fail(FB200_EINVAL, "Please provide excatly one of either SHs or precomputed colors!");
         const bool has_sr = in->d_scales != nullptr && in->d_rotations != nullptr;
         const bool any_sr = in->d_scales != nullptr || in->d_rotations != nullptr;
         const bool has_cov = in->d_cov3D_precomp != nullptr;
         if ((!has_sr && !has_cov) || (any_sr && has_cov))
             return fail(FB200_EINVAL,
-                        "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!%s");
+                        "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
         if (has_sh && (prm->sh_coeffs <= 0 || prm->sh_degree < 0 || prm->sh_degree > 3 ||
                        (prm->sh_degree + 1) * (prm->sh_degree + 1) > prm->sh_coeffs))
-            return fail(FB200_EINVAL, "sh_degree / sh_coeffs inconsistent%s");
+            return fail(FB200_EINVAL, "sh_degree / sh_coeffs inconsistent");
         // rows read with 128-bit loads (header: Alignment)
-        if ((in->d_rotations && (reinterpret_cast<uintptr_t>(in->d_rotations) & 15)) ||
-            (has_sh && (prm->sh_coeffs * 3) % 4 == 0 && (reinterpret_cast<uintptr_t>(in->d_shs) & 15)))
-            return fail(FB200_EINVAL, "rotations / SH rows must be 16-byte aligned%s");
+        if (misaligned(in->d_rotations, 16) || (has_sh && (prm->sh_coeffs * 3) % 4 == 0 && misaligned(in->d_shs, 16)))
+            return fail(FB200_EINVAL, "rotations / SH rows must be 16-byte aligned");
         if ((in->d_point_cells == nullptr) != (in->d_face_visible == nullptr))
-            return fail(FB200_EINVAL, "give both d_point_cells and d_face_visible or neither%s");
+            return fail(FB200_EINVAL, "give both d_point_cells and d_face_visible or neither");
         if (in->d_point_cells && (in->n_cell_points < 0 || in->n_cell_points > prm->P))
-            return fail(FB200_EINVAL, "n_cell_points must be within [0, P]%s");
+            return fail(FB200_EINVAL, "n_cell_points must be within [0, P]");
     }
     if (!in->d_background || !in->d_viewmatrix || !in->d_projmatrix || !in->d_campos)
-        return fail(FB200_EINVAL, "camera tensors missing%s");
-    if (!ws->d_geom || !ws->d_image || !ws->d_status) return fail(FB200_EINVAL, "workspace pointers missing%s");
-    if (ws->binning_capacity > 0 && !ws->d_binning) return fail(FB200_EINVAL, "binning buffer missing%s");
+        return fail(FB200_EINVAL, "camera tensors missing");
+    if (!ws->d_geom || !ws->d_image || !ws->d_status) return fail(FB200_EINVAL, "workspace pointers missing");
+    if (ws->binning_capacity > 0 && !ws->d_binning) return fail(FB200_EINVAL, "binning buffer missing");
     if (ws->binning_capacity < 0 || ws->binning_capacity > 0x7fffffffLL)
-        return fail(FB200_EINVAL, "binning capacity out of range%s");
+        return fail(FB200_EINVAL, "binning capacity out of range");
     const GeomLayout gl((size_t)prm->P);
     const ImageLayout il(prm->image_width, prm->image_height);
     const BinLayout bl((size_t)ws->binning_capacity);
-    if (ws->geom_bytes < gl.total) return fail(FB200_ENOSPC, "geometry workspace too small%s");
-    if (ws->image_bytes < il.total) return fail(FB200_ENOSPC, "image workspace too small%s");
+    if (ws->geom_bytes < gl.total) return fail(FB200_ENOSPC, "geometry workspace too small");
+    if (ws->image_bytes < il.total) return fail(FB200_ENOSPC, "image workspace too small");
     if (ws->binning_capacity > 0 && ws->binning_bytes < bl.total)
-        return fail(FB200_ENOSPC, "binning workspace too small%s");
+        return fail(FB200_ENOSPC, "binning workspace too small");
     return FB200_OK;
 }
 
@@ -171,10 +170,10 @@ int setup_extra(const fb200_params* prm, bool forward, bool backward, ExtraArgs&
     const fb200_extra* e = prm->extra;
     if (!e || prm->P == 0) return FB200_OK;
     if (e->channels < 1 || e->channels > FB200_CHANNELS)
-        return fail(FB200_EINVAL, "extra feature channels must be 1..3%s");
-    if (!e->d_features || !e->d_background) return fail(FB200_EINVAL, "extra features / background missing%s");
-    if (forward && !e->d_out) return fail(FB200_EINVAL, "extra output image missing%s");
-    if (backward && (!e->d_dL_dout || !e->d_dL_dfeatures)) return fail(FB200_EINVAL, "extra gradient pointers missing%s");
+        return fail(FB200_EINVAL, "extra feature channels must be 1..3");
+    if (!e->d_features || !e->d_background) return fail(FB200_EINVAL, "extra features / background missing");
+    if (forward && !e->d_out) return fail(FB200_EINVAL, "extra output image missing");
+    if (backward && (!e->d_dL_dout || !e->d_dL_dfeatures)) return fail(FB200_EINVAL, "extra gradient pointers missing");
     ex.ch = e->channels; ex.feat = e->d_features; ex.bg = e->d_background; ex.out = e->d_out;
     ex.dL_dout = e->d_dL_dout; ex.dL_dfeat = e->d_dL_dfeatures;
     return FB200_OK;
@@ -240,7 +239,7 @@ extern "C" {
 int fb200_profile_enable(int32_t enable) { g_profile.store(enable ? 1 : 0); return FB200_OK; }
 
 int fb200_profile_read(float* ms_out) {
-    if (!ms_out) return fail(FB200_EINVAL, "profile_read: null output%s");
+    if (!ms_out) return fail(FB200_EINVAL, "profile_read: null output");
     std::lock_guard<std::mutex> lk(g_ev_mu);
     for (int i = 0; i < FB200_NUM_STAGES; ++i) {
         ms_out[i] = -1.0f;
@@ -259,10 +258,12 @@ int64_t fb200_kernel_launches(void) { return g_launches.load(); }
 int fb200_abi_version(void) { return FB200_ABI_VERSION; }
 
 int fb200_abi_struct_sizes(size_t* out) {
-    if (!out) return fail(FB200_EINVAL, "abi_struct_sizes: null output%s");
+    if (!out) return fail(FB200_EINVAL, "abi_struct_sizes: null output");
     const size_t sizes[FB200_ABI_STRUCTS] = {sizeof(fb200_params), sizeof(fb200_inputs), sizeof(fb200_workspace),
                                              sizeof(fb200_grads), sizeof(fb200_extra), sizeof(fb200_frosting_params),
-                                             sizeof(fb200_frosting_grads), sizeof(fb200_adam_args), sizeof(fb200_layout)};
+                                             sizeof(fb200_frosting_grads), sizeof(fb200_adam_args), sizeof(fb200_layout),
+                                             sizeof(fb200_frosting_edit), sizeof(fb200_frosting_skin),
+                                             sizeof(fb200_texture), sizeof(fb200_sugar_reg)};
     for (int i = 0; i < FB200_ABI_STRUCTS; ++i) out[i] = sizes[i];
     return FB200_OK;
 }
@@ -273,7 +274,7 @@ size_t fb200_image_bytes(int32_t W, int32_t H) { return ImageLayout(W < 1 ? 1 : 
 size_t fb200_binning_bytes(int64_t capacity) { return BinLayout((size_t)(capacity < 0 ? 0 : capacity)).total; }
 
 int fb200_get_layout(int32_t P, int32_t W, int32_t H, int64_t capacity, fb200_layout* out) {
-    if (!out || P < 0 || W <= 0 || H <= 0 || capacity < 0) return fail(FB200_EINVAL, "bad layout query%s");
+    if (!out || P < 0 || W <= 0 || H <= 0 || capacity < 0) return fail(FB200_EINVAL, "bad layout query");
     const GeomLayout gl((size_t)P);
     const ImageLayout il(W, H);
     const BinLayout bl((size_t)capacity);
@@ -289,8 +290,8 @@ static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb20
                      float* d_out_color, int32_t* d_radii, FwdArgs& a) {
     int rc = validate(prm, in, ws);
     if (rc != FB200_OK) return rc;
-    if (prm->P > 0 && !d_radii) return fail(FB200_EINVAL, "output pointers missing%s");
-    if (need_binning && !d_out_color) return fail(FB200_EINVAL, "output pointers missing%s");
+    if (prm->P > 0 && !d_radii) return fail(FB200_EINVAL, "output pointers missing");
+    if (need_binning && !d_out_color) return fail(FB200_EINVAL, "output pointers missing");
     const GeomLayout gl((size_t)prm->P);
     const ImageLayout il(prm->image_width, prm->image_height);
     const BinLayout bl((size_t)ws->binning_capacity);
@@ -372,7 +373,7 @@ int fb200_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_w
                   float* d_out_color, int32_t* d_radii, void* stream) {
     int rc = fb200_forward_geometry(prm, in, ws, d_radii, stream);
     if (rc != FB200_OK) return rc;
-    if (!ws) return fail(FB200_EINVAL, "null argument struct%s");
+    if (!ws) return fail(FB200_EINVAL, "null argument struct");
     fb200_workspace one_phase = *ws;
     one_phase.h_status = nullptr;      // nobody has synchronised: the host cannot know this frame's status words
     return fb200_forward_raster(prm, in, &one_phase, d_out_color, d_radii, stream);
@@ -382,22 +383,21 @@ int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_
                    const int32_t* d_radii, const float* d_dL_dout_color, const fb200_grads* grads, void* stream) {
     int rc = validate(prm, in, ws);
     if (rc != FB200_OK) return rc;
-    if (!grads || !d_dL_dout_color || (prm->P > 0 && !d_radii)) return fail(FB200_EINVAL, "backward pointers missing%s");
+    if (!grads || !d_dL_dout_color || (prm->P > 0 && !d_radii)) return fail(FB200_EINVAL, "backward pointers missing");
     // outputs a caller cannot use may be NULL and are then not written: dL/dcolors on the SH path (an intermediate
     // there), dL/dcov3D on the scale/rotation path, dL/dscales + dL/drotations on the precomputed-covariance path
     const fb200_frosting_grads* fg = grads->frosting;
     if (in->frosting) {
         if ((rc = check_frosting_grads(in->frosting, fg)) != FB200_OK) return rc;
     } else if (fg) {
-        return fail(FB200_EINVAL, "fb200_grads.frosting given without fb200_inputs.frosting%s");
+        return fail(FB200_EINVAL, "fb200_grads.frosting given without fb200_inputs.frosting");
     } else if (prm->P > 0 && (!grads->d_dL_dmeans2D || !grads->d_dL_dopacity || !grads->d_dL_dmeans3D ||
                        (in->d_colors_precomp && !grads->d_dL_dcolors) || (in->d_cov3D_precomp && !grads->d_dL_dcov3D) ||
                        (!in->d_cov3D_precomp && (!grads->d_dL_dscales || !grads->d_dL_drotations)) ||
                        (in->d_shs && prm->sh_coeffs > 0 && !grads->d_dL_dsh)))
-        return fail(FB200_EINVAL, "gradient output pointers missing%s");
-    if ((grads->d_dL_drotations && (reinterpret_cast<uintptr_t>(grads->d_dL_drotations) & 15)) ||
-        (grads->d_dL_dsh && (prm->sh_coeffs * 3) % 4 == 0 && (reinterpret_cast<uintptr_t>(grads->d_dL_dsh) & 15)))
-        return fail(FB200_EINVAL, "dL/drotations / dL/dsh rows must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "gradient output pointers missing");
+    if (misaligned(grads->d_dL_drotations, 16) || ((prm->sh_coeffs * 3) % 4 == 0 && misaligned(grads->d_dL_dsh, 16)))
+        return fail(FB200_EINVAL, "dL/drotations / dL/dsh rows must be 16-byte aligned");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bool debug = (prm->debug & 1) != 0;
     if (prm->P == 0) return FB200_OK;
@@ -446,7 +446,7 @@ int fb200_mark_visible(int32_t P, const float* d_means3D, const float* d_viewmat
                        uint8_t* d_present, void* stream) {
     (void)d_projmatrix;   // the reference's x/y frustum test is commented out (auxiliary.h:154)
     if (P < 0 || (P > 0 && (!d_means3D || !d_viewmatrix || !d_present)))
-        return fail(FB200_EINVAL, "mark_visible: bad arguments%s");
+        return fail(FB200_EINVAL, "mark_visible: bad arguments");
     return check(launch_mark_visible(P, d_means3D, d_viewmatrix, d_present, static_cast<cudaStream_t>(stream)),
                  "mark_visible");
 }
@@ -457,7 +457,7 @@ int fb200_mesh_visibility(int32_t V, int32_t F, const float* d_verts, const int3
                           int32_t* d_scratch, void* stream) {
     if (V < 0 || F < 0 || W <= 0 || H <= 0 || !d_full_proj || !d_zbuf || !d_pix_to_face ||
         (F > 0 && (!d_verts || !d_faces)))
-        return fail(FB200_EINVAL, "mesh_visibility: bad arguments%s");
+        return fail(FB200_EINVAL, "mesh_visibility: bad arguments");
     return check(launch_mesh_visibility(V, F, d_verts, d_faces, d_full_proj, W, H,
                                         reinterpret_cast<unsigned long long*>(d_zbuf), d_pix_to_face,
                                         d_face_visible, mark_last_on_bg, d_scratch, static_cast<cudaStream_t>(stream)),
@@ -469,7 +469,7 @@ int fb200_gaussian_mask_from_faces(int32_t n_points, const int64_t* d_point_cell
                                    void* stream) {
     if (n_points < 0 || n_background < 0 || F < 0 || (n_points > 0 && (!d_point_cell_indices || !d_face_visible)) ||
         (n_points + n_background > 0 && !d_mask))
-        return fail(FB200_EINVAL, "gaussian_mask_from_faces: bad arguments%s");
+        return fail(FB200_EINVAL, "gaussian_mask_from_faces: bad arguments");
     return check(launch_mask_from_faces(n_points, reinterpret_cast<const long long*>(d_point_cell_indices), F,
                                         d_face_visible, n_background, d_mask, static_cast<cudaStream_t>(stream)),
                  "gaussian_mask_from_faces");
@@ -481,12 +481,12 @@ int fb200_frosting_attributes(const fb200_frosting_params* fp, float* d_means3D,
     if (rc != FB200_OK) return rc;
     const bool rows = (int64_t)fp->P + fp->n_bg > 0;
     if (rows && (!d_means3D || !d_opacities || !d_scales || !d_rotations || !d_shs))
-        return fail(FB200_EINVAL, "frosting_attributes: missing output pointer%s");
+        return fail(FB200_EINVAL, "frosting_attributes: missing output pointer");
     // mesh rows of 16 SH coefficients are stored as twelve float4
     if (fp->P > 0 && fp->sh_rest == 15 && misaligned(d_shs, 16))
-        return fail(FB200_EINVAL, "frosting_attributes: shs must be 16-byte aligned when sh_rest == 15%s");
+        return fail(FB200_EINVAL, "frosting_attributes: shs must be 16-byte aligned when sh_rest == 15");
     if (rows && misaligned(d_rotations, 16))
-        return fail(FB200_EINVAL, "frosting_attributes: rotations must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting_attributes: rotations must be 16-byte aligned");
     return check(launch_frosting_attr_fwd(*fp, d_means3D, d_opacities, d_scales, d_rotations, d_shs,
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes");
 }
@@ -500,44 +500,42 @@ int fb200_frosting_attributes_backward(const fb200_frosting_params* fp, const fl
     if ((rc = check_frosting_grads(fp, grads)) != FB200_OK) return rc;
     const bool rows = (int64_t)fp->P + fp->n_bg > 0;
     if (rows && (!d_g_means3D || !d_g_opacities || !d_g_scales || !d_g_rotations || !d_g_shs))
-        return fail(FB200_EINVAL, "frosting_attributes_backward: missing upstream gradient pointer%s");
+        return fail(FB200_EINVAL, "frosting_attributes_backward: missing upstream gradient pointer");
     // mesh rows of 16 SH coefficients are read as twelve float4
     if (fp->P > 0 && fp->sh_rest == 15 && misaligned(d_g_shs, 16))
-        return fail(FB200_EINVAL, "frosting_attributes_backward: dL/dshs must be 16-byte aligned when sh_rest == 15%s");
+        return fail(FB200_EINVAL, "frosting_attributes_backward: dL/dshs must be 16-byte aligned when sh_rest == 15");
     if (rows && misaligned(d_g_rotations, 16))
-        return fail(FB200_EINVAL, "frosting_attributes_backward: dL/drotations must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting_attributes_backward: dL/drotations must be 16-byte aligned");
     return check(launch_frosting_attr_bwd(*fp, d_g_means3D, d_g_opacities, d_g_scales, d_g_rotations, d_g_shs, *grads,
                                           static_cast<cudaStream_t>(stream)), "frosting_attributes_backward");
 }
 
 static int check_edit(const fb200_frosting_edit* e) {
-    if (!e) return fail(FB200_EINVAL, "frosting_edit: null edit struct%s");
+    if (!e) return fail(FB200_EINVAL, "frosting_edit: null edit struct");
     if (e->n_verts < 0 || e->n_faces < 0 || e->n_edited < 0 || e->n_edited > e->n_faces)
-        return fail(FB200_EINVAL, "frosting_edit: bad extents%s");
+        return fail(FB200_EINVAL, "frosting_edit: bad extents");
     if (e->rescaling != FB200_RESCALE_MEDIAN && e->rescaling != FB200_RESCALE_TRIANGLE)
-        return fail(FB200_EINVAL, "frosting_edit: unknown thickness rescaling method (median = 0, triangle = 1)%s");
+        return fail(FB200_EINVAL, "frosting_edit: unknown thickness rescaling method (median = 0, triangle = 1)");
     if (e->n_faces > 0 && (!e->d_base_verts || !e->d_faces || !e->d_edition_mask || !e->d_dists || !e->d_face_normals ||
                            !e->d_rel_quats || !e->d_face_factor || !e->d_face_keep))
-        return fail(FB200_EINVAL, "frosting_edit: missing face table pointer%s");
+        return fail(FB200_EINVAL, "frosting_edit: missing face table pointer");
     if (e->n_verts > 0 && (!e->d_inner_dist || !e->d_outer_dist || !e->d_verts_edition_mask || !e->d_vf_offsets ||
                            !e->d_vf_faces || !e->d_inner_verts || !e->d_outer_verts))
-        return fail(FB200_EINVAL, "frosting_edit: missing vertex table pointer%s");
-    if (!e->d_factor || !e->d_select) return fail(FB200_EINVAL, "frosting_edit: missing factor / select scratch%s");
+        return fail(FB200_EINVAL, "frosting_edit: missing vertex table pointer");
+    if (!e->d_factor || !e->d_select) return fail(FB200_EINVAL, "frosting_edit: missing factor / select scratch");
     const bool capture = !e->d_ref_quats && !e->d_ref_dists && !e->d_ref_median;
     if (!capture && (!e->d_ref_quats || !e->d_ref_dists || (e->rescaling == FB200_RESCALE_MEDIAN && !e->d_ref_median)))
-        return fail(FB200_EINVAL, "frosting_edit: give every reference table (or none to capture one)%s");
-    if ((reinterpret_cast<uintptr_t>(e->d_rel_quats) & 15) || (reinterpret_cast<uintptr_t>(e->d_ref_quats) & 15))
-        return fail(FB200_EINVAL, "frosting_edit: quaternion tables must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting_edit: give every reference table (or none to capture one)");
+    if (misaligned(e->d_rel_quats, 16) || misaligned(e->d_ref_quats, 16))
+        return fail(FB200_EINVAL, "frosting_edit: quaternion tables must be 16-byte aligned");
     return FB200_OK;
 }
-
-size_t fb200_frosting_edit_struct_size(void) { return sizeof(fb200_frosting_edit); }
 
 int fb200_frosting_edit_shell(const fb200_frosting_edit* e, void* stream) {
     int rc = check_edit(e);
     if (rc != FB200_OK) return rc;
     if (e->rescaling == FB200_RESCALE_MEDIAN && e->n_edited == 0)
-        return fail(FB200_EINVAL, "frosting_edit: median rescaling needs at least one edited face%s");
+        return fail(FB200_EINVAL, "frosting_edit: median rescaling needs at least one edited face");
     return check(launch_frosting_edit_shell(*e, static_cast<cudaStream_t>(stream)), "frosting_edit_shell");
 }
 
@@ -547,7 +545,7 @@ static int check_edit_block(const fb200_frosting_edit* e, const fb200_frosting_p
     if (rc != FB200_OK) return rc;
     if ((rc = check_frosting(fp)) != FB200_OK) return rc;
     if (fp->n_faces != e->n_faces || fp->n_verts != e->n_verts)
-        return fail(FB200_EINVAL, "frosting_edit: the parameter block's mesh does not match the edit's%s");
+        return fail(FB200_EINVAL, "frosting_edit: the parameter block's mesh does not match the edit's");
     return FB200_OK;
 }
 
@@ -557,12 +555,12 @@ static int check_edit_attributes(const fb200_frosting_edit* e, const fb200_frost
     int rc = check_edit_block(e, fp);
     if (rc != FB200_OK) return rc;
     if (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > fp->sh_rest + 1)
-        return fail(FB200_EINVAL, "frosting_edit: sh_degree needs (sh_degree + 1)^2 <= sh_rest + 1 <= 16%s");
+        return fail(FB200_EINVAL, "frosting_edit: sh_degree needs (sh_degree + 1)^2 <= sh_rest + 1 <= 16");
     const bool rows = (int64_t)fp->P + fp->n_bg > 0;
     if (rows && (!d_campos || !d_means3D || !d_opacities || !d_scales || !d_rotations || !d_colors))
-        return fail(FB200_EINVAL, "frosting_edit: missing output pointer%s");
-    if ((reinterpret_cast<uintptr_t>(d_rotations) & 15) || (reinterpret_cast<uintptr_t>(d_orig_quats) & 15))
-        return fail(FB200_EINVAL, "frosting_edit: rotations / orig quats must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting_edit: missing output pointer");
+    if (misaligned(d_rotations, 16) || misaligned(d_orig_quats, 16))
+        return fail(FB200_EINVAL, "frosting_edit: rotations / orig quats must be 16-byte aligned");
     return FB200_OK;
 }
 
@@ -581,8 +579,8 @@ int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_fro
 // the complex adaptation's tables: [F,9] cell transforms when a face is edited, [P,9] canonical transforms
 static int check_edit_complex(const fb200_frosting_edit* e, const fb200_frosting_params* fp, const float* d_cell_T,
                               const float* d_canonical) {
-    if (e->n_edited > 0 && !d_cell_T) return fail(FB200_EINVAL, "frosting_edit_complex: missing cell transforms%s");
-    if (fp->P > 0 && !d_canonical) return fail(FB200_EINVAL, "frosting_edit_complex: missing canonical transforms%s");
+    if (e->n_edited > 0 && !d_cell_T) return fail(FB200_EINVAL, "frosting_edit_complex: missing cell transforms");
+    if (fp->P > 0 && !d_canonical) return fail(FB200_EINVAL, "frosting_edit_complex: missing canonical transforms");
     return FB200_OK;
 }
 
@@ -591,7 +589,7 @@ int fb200_frosting_edit_complex_capture(const fb200_frosting_edit* e, const fb20
     int rc = check_edit_block(e, fp);
     if (rc != FB200_OK) return rc;
     if ((rc = check_edit_complex(e, fp, d_cell_T, d_canonical)) != FB200_OK) return rc;
-    if (!d_n_singular) return fail(FB200_EINVAL, "frosting_edit_complex: missing singular-cell counter%s");
+    if (!d_n_singular) return fail(FB200_EINVAL, "frosting_edit_complex: missing singular-cell counter");
     return check(launch_frosting_edit_complex_capture(*e, *fp, d_cell_T, d_canonical, d_n_singular,
                                                       static_cast<cudaStream_t>(stream)),
                  "frosting_edit_complex_capture");
@@ -612,20 +610,18 @@ int fb200_frosting_edit_attributes_complex(const fb200_frosting_edit* e, const f
                  "frosting_edit_attributes_complex");
 }
 
-size_t fb200_frosting_skin_struct_size(void) { return sizeof(fb200_frosting_skin); }
-
 int fb200_frosting_skin_pose(const fb200_frosting_skin* s, int32_t frame, float* d_base_verts, void* stream) {
-    if (!s) return fail(FB200_EINVAL, "frosting_skin: null skin struct%s");
+    if (!s) return fail(FB200_EINVAL, "frosting_skin: null skin struct");
     if (s->n_rows < 0 || s->n_verts < 0 || s->n_bones < 0 || s->n_frames < 0 || s->n_rows > s->n_verts)
-        return fail(FB200_EINVAL, "frosting_skin: bad extents%s");
+        return fail(FB200_EINVAL, "frosting_skin: bad extents");
     if (frame < 0 || frame >= s->n_frames)
-        return fail(FB200_EINVAL, "frosting_skin: frame outside [0, n_frames)%s");
+        return fail(FB200_EINVAL, "frosting_skin: frame outside [0, n_frames)");
     if (s->n_rows > 0 && (!s->d_tpose || !s->d_vert_ids || !s->d_offsets || !d_base_verts))
-        return fail(FB200_EINVAL, "frosting_skin: missing vertex table pointer%s");
+        return fail(FB200_EINVAL, "frosting_skin: missing vertex table pointer");
     if (s->n_rows > 0 && s->n_bones > 0 && (!s->d_bones || !s->d_weights || !s->d_reset || !s->d_pose))
-        return fail(FB200_EINVAL, "frosting_skin: missing bone table pointer%s");
-    if ((reinterpret_cast<uintptr_t>(s->d_reset) & 15) || (reinterpret_cast<uintptr_t>(s->d_pose) & 15))
-        return fail(FB200_EINVAL, "frosting_skin: reset / pose matrices must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "frosting_skin: missing bone table pointer");
+    if (misaligned(s->d_reset, 16) || misaligned(s->d_pose, 16))
+        return fail(FB200_EINVAL, "frosting_skin: reset / pose matrices must be 16-byte aligned");
     if (s->n_rows == 0) return FB200_OK;
     return check(launch_frosting_skin(*s, frame, d_base_verts, static_cast<cudaStream_t>(stream)),
                  "frosting_skin_pose");
@@ -636,28 +632,26 @@ int fb200_mesh_barycentrics(int32_t V, int32_t F, const float* d_verts, const in
                             float* d_bary, void* stream) {
     if (V < 0 || F < 0 || W <= 0 || H <= 0 || (int64_t)W * H > INT32_MAX || !d_full_proj || !d_pix_to_face ||
         !d_bary || (F > 0 && (!d_verts || !d_faces)))
-        return fail(FB200_EINVAL, "mesh_barycentrics: bad arguments%s");
+        return fail(FB200_EINVAL, "mesh_barycentrics: bad arguments");
     return check(launch_mesh_bary(F, d_verts, d_faces, d_full_proj, W, H, d_pix_to_face, d_bary,
                                   static_cast<cudaStream_t>(stream)),
                  "mesh_barycentrics");
 }
 
-size_t fb200_texture_struct_size(void) { return sizeof(fb200_texture); }
-
 namespace {
 
 int check_texture(const fb200_texture* t) {
-    if (!t) return fail(FB200_EINVAL, "texture: null texture struct%s");
+    if (!t) return fail(FB200_EINVAL, "texture: null texture struct");
     const int64_t n = t->n_square_per_axis;
     if (t->n_faces < 1 || t->n_points < 0 || t->square_size < 3 || n < 1 || 2 * n * n < t->n_faces ||
         (int64_t)t->square_size * n != t->texture_size || (int64_t)t->texture_size * t->texture_size > INT32_MAX)
-        return fail(FB200_EINVAL, "texture: bad extents (F >= 1, square_size >= 3, 2 n^2 >= F, T = square_size n)%s");
+        return fail(FB200_EINVAL, "texture: bad extents (F >= 1, square_size >= 3, 2 n^2 >= F, T = square_size n)");
     if (!t->d_cell_offsets || (t->n_points > 0 && (!t->d_cell_points || !t->d_sh_dc)) || !t->d_face_sh)
-        return fail(FB200_EINVAL, "texture: missing face table pointer%s");
+        return fail(FB200_EINVAL, "texture: missing face table pointer");
     if (!t->d_face_acc || !t->d_texel_acc || !t->d_face_winner || !t->d_texel_winner)
-        return fail(FB200_EINVAL, "texture: missing accumulator / winner pointer%s");
-    if ((reinterpret_cast<uintptr_t>(t->d_face_acc) & 15) || (reinterpret_cast<uintptr_t>(t->d_texel_acc) & 15))
-        return fail(FB200_EINVAL, "texture: accumulators must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "texture: missing accumulator / winner pointer");
+    if (misaligned(t->d_face_acc, 16) || misaligned(t->d_texel_acc, 16))
+        return fail(FB200_EINVAL, "texture: accumulators must be 16-byte aligned");
     return FB200_OK;
 }
 
@@ -674,7 +668,7 @@ int fb200_texture_add_view(const fb200_texture* t, const float* d_image, const i
     int rc = check_texture(t);
     if (rc != FB200_OK) return rc;
     if (W <= 0 || H <= 0 || (int64_t)W * H > INT32_MAX || !d_image || !d_pix_to_face || !d_bary)
-        return fail(FB200_EINVAL, "texture_add_view: bad arguments%s");
+        return fail(FB200_EINVAL, "texture_add_view: bad arguments");
     return check(launch_texture_add_view(*t, d_image, d_pix_to_face, d_bary, W * H, static_cast<cudaStream_t>(stream)),
                  "texture_add_view");
 }
@@ -682,7 +676,7 @@ int fb200_texture_add_view(const fb200_texture* t, const float* d_image, const i
 int fb200_texture_finish(const fb200_texture* t, float* d_texture, void* stream) {
     int rc = check_texture(t);
     if (rc != FB200_OK) return rc;
-    if (!d_texture) return fail(FB200_EINVAL, "texture_finish: missing output%s");
+    if (!d_texture) return fail(FB200_EINVAL, "texture_finish: missing output");
     return check(launch_texture_fill(*t, d_texture, static_cast<cudaStream_t>(stream)), "texture_finish");
 }
 
@@ -693,7 +687,7 @@ size_t fb200_loss_partials(int32_t C, int32_t H, int32_t W) {
 int fb200_l1_dssim_forward(const float* d_pred, const float* d_gt, int32_t C, int32_t H, int32_t W, float lambda,
                            float* d_maps, float* d_partials, float* d_loss, void* stream) {
     if (C <= 0 || H <= 0 || W <= 0 || !d_pred || !d_gt || !d_maps || !d_partials || !d_loss)
-        return fail(FB200_EINVAL, "l1_dssim_forward: bad arguments%s");
+        return fail(FB200_EINVAL, "l1_dssim_forward: bad arguments");
     return check(launch_l1_dssim_fwd(d_pred, d_gt, C, H, W, lambda, d_maps, d_partials, d_loss,
                                      static_cast<cudaStream_t>(stream)), "l1_dssim_forward");
 }
@@ -701,35 +695,33 @@ int fb200_l1_dssim_forward(const float* d_pred, const float* d_gt, int32_t C, in
 int fb200_l1_dssim_backward(const float* d_pred, const float* d_gt, const float* d_maps, int32_t C, int32_t H,
                             int32_t W, float lambda, const float* d_dL_dloss, float* d_dpred, void* stream) {
     if (C <= 0 || H <= 0 || W <= 0 || !d_pred || !d_gt || !d_maps || !d_dL_dloss || !d_dpred)
-        return fail(FB200_EINVAL, "l1_dssim_backward: bad arguments%s");
+        return fail(FB200_EINVAL, "l1_dssim_backward: bad arguments");
     return check(launch_l1_dssim_bwd(d_pred, d_gt, d_maps, C, H, W, lambda, d_dL_dloss, d_dpred,
                                      static_cast<cudaStream_t>(stream)), "l1_dssim_backward");
 }
-
-size_t fb200_sugar_reg_struct_size(void) { return sizeof(fb200_sugar_reg); }
 
 size_t fb200_sugar_reg_workspace_bytes(int32_t P, int32_t K, int32_t N, int32_t with_grad) {
     return (P >= 0 && K >= 1 && K <= 32 && N >= 0) ? sugar_reg_workspace_bytes(P, K, N, with_grad != 0) : 0;
 }
 
 static int check_sugar_reg(const fb200_sugar_reg* r) {
-    if (!r) return fail(FB200_EINVAL, "sugar_reg: null struct%s");
+    if (!r) return fail(FB200_EINVAL, "sugar_reg: null struct");
     if (r->P < 0 || r->N < 0 || (r->N > 0 && r->P == 0))
-        return fail(FB200_EINVAL, "sugar_reg: bad extents (P >= 0, N >= 0, P > 0 when N > 0)%s");
-    if (r->K < 1 || r->K > 32) return fail(FB200_EINVAL, "sugar_reg: K must be within [1, 32]%s");
-    if (!r->d_workspace) return fail(FB200_EINVAL, "sugar_reg: missing workspace%s");
+        return fail(FB200_EINVAL, "sugar_reg: bad extents (P >= 0, N >= 0, P > 0 when N > 0)");
+    if (r->K < 1 || r->K > 32) return fail(FB200_EINVAL, "sugar_reg: K must be within [1, 32]");
+    if (!r->d_workspace) return fail(FB200_EINVAL, "sugar_reg: missing workspace");
     if (r->P > 0 && (!r->d_points || !r->d_scaling || !r->d_quaternions || !r->d_strengths || !r->d_knn_idx))
-        return fail(FB200_EINVAL, "sugar_reg: missing Gaussian pointer%s");
-    if (r->N > 0 && (!r->d_idx || !r->d_eps)) return fail(FB200_EINVAL, "sugar_reg: missing sample pointer%s");
+        return fail(FB200_EINVAL, "sugar_reg: missing Gaussian pointer");
+    if (r->N > 0 && (!r->d_idx || !r->d_eps)) return fail(FB200_EINVAL, "sugar_reg: missing sample pointer");
     if (misaligned(r->d_quaternions, 16) || misaligned(r->d_workspace, 16))
-        return fail(FB200_EINVAL, "sugar_reg: quaternions and workspace must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "sugar_reg: quaternions and workspace must be 16-byte aligned");
     return FB200_OK;
 }
 
 int fb200_sugar_reg_forward(const fb200_sugar_reg* r, int32_t with_grad, float* d_terms, void* stream) {
     int rc = check_sugar_reg(r);
     if (rc != FB200_OK) return rc;
-    if (!d_terms) return fail(FB200_EINVAL, "sugar_reg_forward: missing terms output%s");
+    if (!d_terms) return fail(FB200_EINVAL, "sugar_reg_forward: missing terms output");
     return check(launch_sugar_reg_fwd(*r, with_grad != 0, d_terms, static_cast<cudaStream_t>(stream)),
                  "sugar_reg_forward");
 }
@@ -740,53 +732,53 @@ int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms,
     if (rc != FB200_OK) return rc;
     if (r->P == 0) return FB200_OK;
     if (!d_dL_dterms || !d_dpoints || !d_dscaling || !d_dquaternions || !d_dstrengths)
-        return fail(FB200_EINVAL, "sugar_reg_backward: missing gradient pointer%s");
+        return fail(FB200_EINVAL, "sugar_reg_backward: missing gradient pointer");
     if (misaligned(d_dquaternions, 16))
-        return fail(FB200_EINVAL, "sugar_reg_backward: dL/dquaternions must be 16-byte aligned%s");
+        return fail(FB200_EINVAL, "sugar_reg_backward: dL/dquaternions must be 16-byte aligned");
     return check(launch_sugar_reg_bwd(*r, d_dL_dterms, d_dpoints, d_dscaling, d_dquaternions, d_dstrengths,
                                       static_cast<cudaStream_t>(stream)),
                  "sugar_reg_backward");
 }
 
 int fb200_adam_step(const fb200_adam_args* a, void* stream) {
-    if (!a) return fail(FB200_EINVAL, "adam_step: null args%s");
+    if (!a) return fail(FB200_EINVAL, "adam_step: null args");
     if (a->world < 1 || a->world > FB200_MAX_PEERS || a->rank < 0 || a->rank >= a->world)
-        return fail(FB200_EINVAL, "adam_step: world must be 1..8 and rank inside it%s");
+        return fail(FB200_EINVAL, "adam_step: world must be 1..8 and rank inside it");
     if (a->n_groups < 1 || a->n_groups > FB200_ADAM_MAX_GROUPS)
-        return fail(FB200_EINVAL, "adam_step: 1..16 parameter groups%s");
+        return fail(FB200_EINVAL, "adam_step: 1..16 parameter groups");
     for (int g = 0; g <= a->n_groups; ++g)
         if ((a->group_start[g] & 3) || (g > 0 && a->group_start[g] < a->group_start[g - 1]))
-            return fail(FB200_EINVAL, "adam_step: group starts must be ascending multiples of 4 elements%s");
+            return fail(FB200_EINVAL, "adam_step: group starts must be ascending multiples of 4 elements");
     if ((a->shard_lo & 3) || (a->shard_hi & 3) || a->shard_lo < a->group_start[0] || a->shard_hi < a->shard_lo ||
         a->shard_hi > a->group_start[a->n_groups])
-        return fail(FB200_EINVAL, "adam_step: shard must be a 4-aligned range inside the slab%s");
+        return fail(FB200_EINVAL, "adam_step: shard must be a 4-aligned range inside the slab");
     if (a->shard_hi > a->shard_lo) {
-        if (!a->d_exp_avg || !a->d_exp_avg_sq) return fail(FB200_EINVAL, "adam_step: missing moment buffers%s");
+        if (!a->d_exp_avg || !a->d_exp_avg_sq) return fail(FB200_EINVAL, "adam_step: missing moment buffers");
         for (int p = 0; p < a->world; ++p)
-            if (!a->peer_params[p] || !a->peer_grads[p]) return fail(FB200_EINVAL, "adam_step: missing slab pointer%s");
+            if (!a->peer_params[p] || !a->peer_grads[p]) return fail(FB200_EINVAL, "adam_step: missing slab pointer");
     }
     if ((a->mc_grads == nullptr) != (a->mc_params == nullptr))
-        return fail(FB200_EINVAL, "adam_step: give both multicast mappings or neither%s");
+        return fail(FB200_EINVAL, "adam_step: give both multicast mappings or neither");
     {
         int given = 0;
         for (int p = 0; p < a->world; ++p) given += a->peer_row_radii[p] != nullptr;
-        if (given != 0 && given != a->world) return fail(FB200_EINVAL, "adam_step: give every rank's row radii or none%s");
+        if (given != 0 && given != a->world) return fail(FB200_EINVAL, "adam_step: give every rank's row radii or none");
         if (given) {
-            if (a->row_count < 1) return fail(FB200_EINVAL, "adam_step: row_count must be positive with row radii%s");
+            if (a->row_count < 1) return fail(FB200_EINVAL, "adam_step: row_count must be positive with row radii");
             for (int g = 0; g < a->n_groups; ++g) {
                 const int64_t n = a->group_start[g + 1] - a->group_start[g];
                 if (a->row_width[g] < 0 || (int64_t)a->row_width[g] * a->row_count > n || n > 0xffffffffLL)
-                    return fail(FB200_EINVAL, "adam_step: row_width * row_count exceeds the group%s");
+                    return fail(FB200_EINVAL, "adam_step: row_width * row_count exceeds the group");
             }
         }
     }
     if (!(a->bias_correction1 > 0.f) || !(a->bias_correction2_sqrt > 0.f))
-        return fail(FB200_EINVAL, "adam_step: bias corrections must be positive (step >= 1)%s");
+        return fail(FB200_EINVAL, "adam_step: bias corrections must be positive (step >= 1)");
     return check(launch_adam_shard(*a, static_cast<cudaStream_t>(stream)), "adam_step");
 }
 
 int fb200_peer_alloc(size_t bytes, void** d_ptr) {
-    if (!d_ptr || bytes == 0) return fail(FB200_EINVAL, "peer_alloc: bad arguments%s");
+    if (!d_ptr || bytes == 0) return fail(FB200_EINVAL, "peer_alloc: bad arguments");
     void* p = nullptr;
     int rc = check(cudaMalloc(&p, bytes), "peer_alloc");
     if (rc != FB200_OK) return rc;
@@ -800,7 +792,7 @@ int fb200_peer_free(void* d_ptr) { return d_ptr ? check(cudaFree(d_ptr), "peer_f
 
 int fb200_peer_export(void* d_ptr, unsigned char* handle) {
     static_assert(sizeof(cudaIpcMemHandle_t) == FB200_PEER_HANDLE_BYTES, "handle size");
-    if (!d_ptr || !handle) return fail(FB200_EINVAL, "peer_export: bad arguments%s");
+    if (!d_ptr || !handle) return fail(FB200_EINVAL, "peer_export: bad arguments");
     cudaIpcMemHandle_t h;
     int rc = check(cudaIpcGetMemHandle(&h, d_ptr), "peer_export");
     if (rc == FB200_OK) memcpy(handle, &h, sizeof(h));
@@ -808,7 +800,7 @@ int fb200_peer_export(void* d_ptr, unsigned char* handle) {
 }
 
 int fb200_peer_open(const unsigned char* handle, void** d_ptr) {
-    if (!d_ptr || !handle) return fail(FB200_EINVAL, "peer_open: bad arguments%s");
+    if (!d_ptr || !handle) return fail(FB200_EINVAL, "peer_open: bad arguments");
     cudaIpcMemHandle_t h;
     memcpy(&h, handle, sizeof(h));
     return check(cudaIpcOpenMemHandle(d_ptr, h, cudaIpcMemLazyEnablePeerAccess), "peer_open");

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define FB200_ABI_VERSION 7
+#define FB200_ABI_VERSION 8
 
 #define FB200_OK 0
 #define FB200_EINVAL (-1)   /* bad argument (shape / null pointer / unsupported channel count) */
@@ -336,8 +336,6 @@ int fb200_frosting_edit_attributes(const fb200_frosting_edit* e, const fb200_fro
                                    const float* d_campos /*[3]*/, const float* d_orig_quats, float* d_means3D,
                                    float* d_opacities, float* d_scales, float* d_rotations, float* d_colors,
                                    void* stream);
-/* sizeof(fb200_frosting_edit), for binding mirrors */
-size_t fb200_frosting_edit_struct_size(void);
 
 /* Complex adaptation (make_editable(use_simple_adapt=False), frosting_model.py:900-967, :1055-1119, :1149-1183): each
  * edited Gaussian keeps a canonical transform C = T_ref[cell]^-1 R(q) diag(exp(s)), where T maps a canonical cell to
@@ -381,8 +379,6 @@ typedef struct fb200_frosting_skin {
 } fb200_frosting_skin;
 /* Writes frame `frame` (in [0, n_frames)) into d_base_verts [n_verts,3] in place.  One launch, no allocation. */
 int fb200_frosting_skin_pose(const fb200_frosting_skin* s, int32_t frame, float* d_base_verts, void* stream);
-/* sizeof(fb200_frosting_skin), for binding mirrors */
-size_t fb200_frosting_skin_struct_size(void);
 
 /* Texture bake of the base mesh (frosting_utils/texture.py:11-181 compute_textured_mesh_for_frosting_mesh).
  *
@@ -420,8 +416,6 @@ int fb200_texture_add_view(const fb200_texture* t, const float* d_image, const i
                            const float* d_bary, int32_t W, int32_t H, void* stream);
 /* d_texture [T,T,3]: filled texels sum / count, others their face's colour; rows flipped (row 0 is v = T-1). */
 int fb200_texture_finish(const fb200_texture* t, float* d_texture, void* stream);
-/* sizeof(fb200_texture), for binding mirrors */
-size_t fb200_texture_struct_size(void);
 
 /* Fused photometric loss (1 - lambda) * mean|x - y| + lambda * (1 - SSIM(x, y)) of Frosting's trainers
  * (frosting_utils/loss_utils.py:17-63 with refine.py:407-409; 11x11 Gaussian window, sigma 1.5, zero padding).
@@ -470,8 +464,6 @@ int fb200_sugar_reg_forward(const fb200_sugar_reg* r, int32_t with_grad, float* 
 /* d_dquaternions 16-byte aligned.  Needs a preceding fb200_sugar_reg_forward with_grad on the same workspace. */
 int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms, float* d_dpoints, float* d_dscaling,
                              float* d_dquaternions, float* d_dstrengths, void* stream);
-/* sizeof(fb200_sugar_reg), for binding mirrors */
-size_t fb200_sugar_reg_struct_size(void);
 
 /* Data-parallel gradient reduction fused with the Adam update (SURVEY.md row f3).  Replaces "all-reduce every
  * .grad, then torch.optim.Adam(l, lr=0.0, eps=1e-15).step()" (frosting_scene/frosting_optimizer.py:101,116-118) for
@@ -571,8 +563,9 @@ int64_t fb200_kernel_launches(void);
 const char* fb200_last_error(void);
 int fb200_abi_version(void);
 /* sizeof() of the ABI structs, in this order: {params, inputs, workspace, grads, extra, frosting_params,
- * frosting_grads, adam_args, layout}: lets a foreign-language binding verify its struct mirrors at load time. */
-#define FB200_ABI_STRUCTS 9
+ * frosting_grads, adam_args, layout, frosting_edit, frosting_skin, texture, sugar_reg}: lets a foreign-language binding
+ * verify its struct mirrors at load time.  Check fb200_abi_version() first: the count grows with the version. */
+#define FB200_ABI_STRUCTS 13
 int fb200_abi_struct_sizes(size_t* out /* [FB200_ABI_STRUCTS] */);
 
 #ifdef __cplusplus

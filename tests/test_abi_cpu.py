@@ -10,20 +10,75 @@ from frosting_b200 import _lib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def header_functions():
+def header_source():
     src = open(os.path.join(ROOT, "include", "frosting_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(fb200_[a-z_0-9]+)\s*\(", src)))
+    return re.sub(r"/\*.*?\*/", "", src, flags=re.S)
 
 
-def test_every_declared_symbol_is_exported():
+def header_functions():
+    return sorted(set(re.findall(r"\b(fb200_[a-z_0-9]+)\s*\(", header_source())))
+
+
+def header_prototypes():
+    """name -> (return type, [parameter types]) of every function the header declares; a type is (base, pointer depth)
+    with `const` dropped, e.g. `const float* d_x` -> ("float", 1); `(void)` -> []."""
+    src = re.sub(r"^\s*#.*$", "", header_source(), flags=re.M)
+
+    def ctype(decl):
+        words = decl.replace("*", " ").split()
+        if len(words) > 1 and not decl.rstrip().endswith("*"):
+            words = words[:-1]                                   # the parameter's name
+        return " ".join(w for w in words if w != "const"), decl.count("*")
+
+    out = {}
+    for ret, name, params in re.findall(r"([\w\s*]+?)\b(fb200_\w+)\s*\(([^;{}()]*)\)\s*;", src):
+        params = [] if params.strip() == "void" else [ctype(p) for p in params.split(",")]
+        out[name] = (ctype(ret + " _"), params)
+    return out
+
+
+def test_declared_symbols_are_exported_at_the_pinned_abi_version():
     L = _lib.lib()
     names = header_functions()
     assert len(names) >= 14
     for n in names:
         assert hasattr(L, n), f"{n} declared in the header but not exported"
     assert sorted(_lib.EXPORTED) == names, "frosting_b200/_lib.py:EXPORTED out of sync with the header"
-    assert L.fb200_abi_version() == _lib.ABI_VERSION == 7
+    assert L.fb200_abi_version() == _lib.ABI_VERSION == 8
+    count = re.search(r"#define FB200_ABI_STRUCTS (\d+)", header_source())
+    assert int(count.group(1)) == len(_lib.ABI_STRUCTS)
+
+
+SCALARS = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "size_t": C.c_size_t, "float": C.c_float}
+
+
+def test_binding_matches_every_prototype():
+    """restype and argtypes of each bound function against the header: scalars at their exact ctypes type, fb200_*
+    struct pointers as POINTER(<the struct's mirror>), every other pointer as some pointer type."""
+    L = _lib.lib()
+    mirrors = dict(_lib.ABI_STRUCTS)
+    protos = header_prototypes()
+    assert sorted(protos) == header_functions()
+
+    def mismatch(t, decl):
+        base, depth = decl
+        if depth == 0:
+            return t is not SCALARS[base]
+        if depth == 1 and base in mirrors:
+            return t is not C.POINTER(mirrors[base])
+        return not (isinstance(t, type) and issubclass(t, (C.c_void_p, C.c_char_p, C._Pointer)))
+
+    bad = []
+    for name, (ret, params) in protos.items():
+        fn = getattr(L, name)
+        if mismatch(fn.restype, ret):
+            bad.append(f"{name}: restype {fn.restype} for {ret}")
+        if fn.argtypes is None or len(fn.argtypes) != len(params):
+            bad.append(f"{name}: argtypes {fn.argtypes} for {len(params)} parameters")
+            continue
+        bad += [f"{name}: argument {i} {t} for {p}" for i, (t, p) in enumerate(zip(fn.argtypes, params))
+                if mismatch(t, p)]
+    assert not bad, "\n".join(bad)
 
 
 def test_workspace_size_queries_are_host_only_and_monotonic():

@@ -118,13 +118,11 @@ def test_python_surface_rejects_cpu():
                                  torch.zeros(3, 3))
 
 
-def test_sugar_reg_entry_points_are_exported():
+def test_sugar_reg_entry_points_are_bound():
     import frosting_b200 as fb
     L = _lib.lib()
-    for n in ("fb200_sugar_reg_workspace_bytes", "fb200_sugar_reg_forward", "fb200_sugar_reg_backward",
-              "fb200_sugar_reg_struct_size"):
+    for n in ("fb200_sugar_reg_workspace_bytes", "fb200_sugar_reg_forward", "fb200_sugar_reg_backward"):
         assert n in _lib.EXPORTED and hasattr(L, n)
-    assert L.fb200_sugar_reg_struct_size() == C.sizeof(_lib.SugarReg)
     assert fb.sdf_regularization is sugar.sdf_regularization and fb.SugarNeighbours is sugar.SugarNeighbours
     # records + partials (two floats per block of 16 samples at K = 16, of 32 at K = 5), then with the gradient pass
     # the accumulators from the next 16-byte boundary
