@@ -15,7 +15,7 @@ FB200_STATUS_WORDS = 8
 ST_NUM_RENDERED, ST_OVERFLOW, ST_MAX_TILE, ST_NUM_VISIBLE = 0, 1, 2, 3
 TILE = 16
 NUM_STAGES = 5
-ABI_VERSION = 8
+ABI_VERSION = 9
 STAGES = ("preprocess", "binning", "render_fwd", "render_bwd", "geom_bwd")
 
 
@@ -131,7 +131,7 @@ class AdamArgs(C.Structure):
 class Layout(C.Structure):
     _fields_ = [(n, C.c_size_t) for n in (
         "geom_rec", "geom_depth", "geom_rect", "geom_clamped", "img_final_T", "img_n_contrib",
-        "img_ranges", "img_tile_count", "bin_point_list", "bin_keys", "geom_acc")]
+        "img_ranges", "img_tile_count", "bin_point_list", "bin_keys", "geom_acc", "img_last_entry", "bin_sub_hits")]
 
 
 # (C struct, ctypes mirror) in the order fb200_abi_struct_sizes reports them (FB200_ABI_STRUCTS)

@@ -283,6 +283,7 @@ int fb200_get_layout(int32_t P, int32_t W, int32_t H, int64_t capacity, fb200_la
     out->img_tile_count = il.tile_count;
     out->bin_point_list = bl.point_list; out->bin_keys = bl.keys;
     out->geom_acc = gl.acc;
+    out->img_last_entry = il.last_entry; out->bin_sub_hits = bl.sub_hits;
     return FB200_OK;
 }
 

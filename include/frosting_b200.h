@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define FB200_ABI_VERSION 8
+#define FB200_ABI_VERSION 9
 
 #define FB200_OK 0
 #define FB200_EINVAL (-1)   /* bad argument (shape / null pointer / unsupported channel count) */
@@ -539,6 +539,12 @@ typedef struct fb200_layout {
                               {dmean2D.x, dmean2D.y, dconic.x, dconic.y}, {dconic.w, dopacity, dr, dg}, {db, e0, e1, e2}
                               (e*: extra feature channels).  Valid after fb200_backward until the next forward or
                               backward on the workspace */
+    size_t img_last_entry; /* u32[H*W] per pixel: entries of its sub-tile's hit list up to and including its last
+                              contributor (0: none), written by the forward blend */
+    size_t bin_sub_hits;   /* u32[8*capacity] the hit lists of the 8 sub-tiles (8x4 pixels, row-major: w = 2 * row + col)
+                              of every tile: Gaussian ids that passed the forward's sub-tile test, in tile-list order.
+                              Sub-tile w of a tile with range [s, e) owns entries [8 s + w (e - s), + (e - s)); the first
+                              max(last_entry) of them are valid */
 } fb200_layout;
 
 int fb200_get_layout(int32_t P, int32_t image_width, int32_t image_height, int64_t capacity,

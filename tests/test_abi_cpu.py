@@ -37,14 +37,17 @@ def header_prototypes():
     return out
 
 
-def test_declared_symbols_are_exported_at_the_pinned_abi_version():
+def test_declared_symbols_are_exported_at_the_header_abi_version():
+    """ABI 9: fb200_layout carries the hit lists (img_last_entry, bin_sub_hits).  The library, the binding and the
+    header's FB200_ABI_VERSION agree."""
     L = _lib.lib()
     names = header_functions()
     assert len(names) >= 14
     for n in names:
         assert hasattr(L, n), f"{n} declared in the header but not exported"
     assert sorted(_lib.EXPORTED) == names, "frosting_b200/_lib.py:EXPORTED out of sync with the header"
-    assert L.fb200_abi_version() == _lib.ABI_VERSION == 8
+    version = re.search(r"#define FB200_ABI_VERSION (\d+)", header_source())
+    assert L.fb200_abi_version() == _lib.ABI_VERSION == int(version.group(1)) == 9
     count = re.search(r"#define FB200_ABI_STRUCTS (\d+)", header_source())
     assert int(count.group(1)) == len(_lib.ABI_STRUCTS)
 
@@ -100,8 +103,11 @@ def test_layout_offsets_are_aligned_and_ordered():
     offs = [getattr(lay, n) for n, _ in _lib.Layout._fields_]
     assert all(o % 128 == 0 for o in offs)
     assert lay.geom_rec < lay.geom_depth < lay.geom_rect < lay.geom_clamped < lay.geom_acc
-    assert lay.img_final_T < lay.img_n_contrib < lay.img_ranges < lay.img_tile_count
-    assert lay.bin_point_list < lay.bin_keys
+    assert lay.img_final_T < lay.img_n_contrib < lay.img_last_entry < lay.img_ranges < lay.img_tile_count
+    assert lay.bin_point_list < lay.bin_keys < lay.bin_sub_hits
+    # the two hit-list arrays: one u32 per pixel, eight u32 per instance, both inside their workspaces
+    assert lay.img_ranges - lay.img_last_entry >= 4 * 256 * 128
+    assert lay.bin_sub_hits + 4 * 8 * 5000 <= L.fb200_binning_bytes(5000)
 
 
 def test_argument_errors_are_reported_without_touching_cuda():

@@ -83,3 +83,52 @@ def rel_err_stats(a, b):
     else:
         frac_bad = 0.0
     return max_rel_to_scale, frac_bad
+
+
+def blend_regime_gaussians(P, cam, seed, n_deep=0, device="cpu"):
+    """Free Gaussians (precomputed colours) for the blend kernels' edge cases, built in the view space of `cam` from
+    pixel positions and sizes: an opaque wall of small splats (half of them at opacity > 0.99, i.e. past the 0.99
+    clamp) bounded by a slanted sharp edge, so that sub-tiles on the edge hold saturated and never-saturating pixels
+    side by side; a cloud of anisotropic splats of opacity 0.02 .. 0.7 over the middle; ~0.2 % wide faint splats whose
+    opacity is within 2e-3 above 1/255, so that their alpha crosses 1/255 over whole pixel disks; and an empty strip at
+    the right edge (empty sub-tiles).  `n_deep` extra faint splats centred in one tile push its list past 8192
+    entries (the global-memory sort class)."""
+    g = torch.Generator().manual_seed(seed)
+    U = lambda n, lo, hi: lo + (hi - lo) * torch.rand(n, generator=g)
+    W, H = cam.image_width, cam.image_height
+    fx = W / (2 * cam.tanfovx)
+    fy = H / (2 * cam.tanfovy)
+    n_faint = max(P // 500, 20)
+    n_wall = (P - n_faint) * 2 // 5
+    n_cloud = P - n_faint - n_wall
+    u, v, z, sig, op = [], [], [], [], []
+    # the wall: left of the line u = 0.3 W + 0.25 v
+    vw = U(n_wall, 0, H)
+    u.append(U(n_wall, 0, 1) * (0.3 * W + 0.25 * vw)); v.append(vw); z.append(U(n_wall, 3.0, 4.0))
+    sig.append(U(n_wall, 0.8, 2.0))
+    op.append(torch.where(torch.rand(n_wall, generator=g) < 0.5, U(n_wall, 0.993, 1.0), U(n_wall, 0.5, 0.95)))
+    # the cloud, behind the wall's depth range in part
+    u.append(U(n_cloud, 0.2 * W, W - 80)); v.append(U(n_cloud, 0, H)); z.append(U(n_cloud, 2.0, 10.0))
+    sig.append(U(n_cloud, 1.0, 8.0)); op.append(U(n_cloud, 0.02, 0.7))
+    # faint and wide: alpha = op G crosses 1/255 where G = 1/255 / op, within ~0.06 sigma of the centre
+    u.append(U(n_faint, 0.25 * W, W - 100)); v.append(U(n_faint, 10, H - 10)); z.append(U(n_faint, 2.0, 10.0))
+    sig.append(U(n_faint, 30.0, 60.0)); op.append((1.0 / 255.0) * (1 + U(n_faint, 1e-4, 2e-3)))
+    if n_deep:
+        tx = (W // 32) * 16
+        u.append(U(n_deep, tx, tx + 16)); v.append(U(n_deep, 16, 32)); z.append(U(n_deep, 2.0, 10.0))
+        sig.append(U(n_deep, 0.5, 1.5)); op.append(U(n_deep, 0.01, 0.05))
+    u, v, z, sig, op = (torch.cat(a) for a in (u, v, z, sig, op))
+    N = u.shape[0]
+    x = (u - 0.5 * (W - 1)) / fx * z
+    y = (v - 0.5 * (H - 1)) / fy * z
+    scales = (sig * z / fx)[:, None] * torch.exp(0.25 * torch.randn(N, 3, generator=g))
+    q = torch.randn(N, 4, generator=g)
+    rotations = q / q.norm(dim=1, keepdim=True)
+    colors = torch.rand(N, 3, generator=g)
+    perm = torch.randperm(N, generator=g)
+    means = torch.stack([x, y, z], 1)
+    c2w = torch.linalg.inv(cam.w2c.double())
+    means = (torch.cat([means.double(), torch.ones(N, 1, dtype=torch.float64)], 1) @ c2w.t())[:, :3].float()
+    out = dict(means3D=means, scales=scales.float(), rotations=rotations.float(), opacities=op.float()[:, None],
+               colors=colors.float())
+    return {k: v[perm].contiguous().to(device) for k, v in out.items()}
