@@ -4,6 +4,7 @@ There is no fallback: if the CUDA library is missing this module raises at impor
 and every op in this package fails loudly.  PyTorch is used only for device memory and streams.
 """
 import ctypes as C
+import math
 import os
 
 import torch
@@ -132,6 +133,37 @@ class Layout(C.Structure):
     _fields_ = [(n, C.c_size_t) for n in (
         "geom_rec", "geom_depth", "geom_rect", "geom_clamped", "img_final_T", "img_n_contrib",
         "img_ranges", "img_tile_count", "bin_point_list", "bin_keys", "geom_acc", "img_last_entry", "bin_sub_hits")]
+
+
+def workspace_views(geom, image, binning, P, W, H, capacity, R):
+    """Named tensor views of a frame's workspace sub-arrays, as the library carved them: `fb200_get_layout` offsets from
+    each buffer's first 128-byte aligned byte.  The layout follows from `capacity`; the binning views are R entries
+    long.  A buffer given as None contributes no views."""
+    lay = Layout()
+    check(lib().fb200_get_layout(P, W, H, capacity, C.byref(lay)))
+    T = ((W + TILE - 1) // TILE) * ((H + TILE - 1) // TILE)
+    table = (  # name, buffer, fb200_layout field, dtype, shape
+        ("rec", geom, "geom_rec", torch.float32, (P, 12)),
+        ("depth", geom, "geom_depth", torch.float32, (P,)),
+        ("rect", geom, "geom_rect", torch.int32, (P, 2)),
+        ("clamped", geom, "geom_clamped", torch.uint8, (P,)),
+        ("acc", geom, "geom_acc", torch.float32, (P, 12)),
+        ("final_T", image, "img_final_T", torch.float32, (H, W)),
+        ("n_contrib", image, "img_n_contrib", torch.int32, (H, W)),
+        ("last_entry", image, "img_last_entry", torch.int32, (H, W)),
+        ("ranges", image, "img_ranges", torch.int32, (T, 2)),
+        ("tile_count", image, "img_tile_count", torch.int32, (T,)),
+        ("point_list", binning, "bin_point_list", torch.int32, (R,)),
+        ("keys", binning, "bin_keys", torch.int64, (R,)),
+        ("sub_hits", binning, "bin_sub_hits", torch.int32, (8 * R,)),   # 8 sub-tile hit lists per tile
+    )
+    views = {}
+    for name, buf, field, dtype, shape in table:
+        if buf is None:
+            continue
+        start = (-buf.data_ptr()) % 128 + getattr(lay, field)
+        views[name] = buf[start:start + math.prod(shape) * dtype.itemsize].view(dtype).view(shape)
+    return views
 
 
 # (C struct, ctypes mirror) in the order fb200_abi_struct_sizes reports them (FB200_ABI_STRUCTS)

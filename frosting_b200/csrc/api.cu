@@ -154,6 +154,23 @@ int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_worksp
     if (ws->binning_capacity > 0 && !ws->d_binning) return fail(FB200_EINVAL, "binning buffer missing");
     if (ws->binning_capacity < 0 || ws->binning_capacity > 0x7fffffffLL)
         return fail(FB200_EINVAL, "binning capacity out of range");
+    return FB200_OK;
+}
+
+inline char* align128(void* p) {
+    return reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(p) + 127) & ~uintptr_t(127));
+}
+
+// p = the sub-array at byte offset `off` of a 128-byte aligned workspace base; NULL when there is no such workspace
+template <typename T>
+void carve(T*& p, char* base, size_t off) { p = base ? reinterpret_cast<T*>(base + off) : nullptr; }
+
+// One frame's arguments: checks them and the workspace sizes, then fills the header the kernels read and carves the
+// three workspaces into every sub-array pointer (GeomLayout, ImageLayout, BinLayout from 128-byte aligned bases).
+// `a` is value-initialised by the caller.
+int carve_frame(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws, FrameArgs& a) {
+    int rc = validate(prm, in, ws);
+    if (rc != FB200_OK) return rc;
     const GeomLayout gl((size_t)prm->P);
     const ImageLayout il(prm->image_width, prm->image_height);
     const BinLayout bl((size_t)ws->binning_capacity);
@@ -161,6 +178,27 @@ int validate(const fb200_params* prm, const fb200_inputs* in, const fb200_worksp
     if (ws->image_bytes < il.total) return fail(FB200_ENOSPC, "image workspace too small");
     if (ws->binning_capacity > 0 && ws->binning_bytes < bl.total)
         return fail(FB200_ENOSPC, "binning workspace too small");
+    a.prm = *prm;
+    a.in = *in;
+    if (in->frosting) { a.frosting = 1; a.fr = *in->frosting; a.in = frosting_inputs(in); }
+    // focal lengths exactly as rasterizer_impl.cu:222-223
+    a.focal_y = prm->image_height / (2.0f * prm->tanfovy);
+    a.focal_x = prm->image_width / (2.0f * prm->tanfovx);
+    a.tiles_x = il.tiles_x; a.tiles_y = il.tiles_y;
+    char* g = align128(ws->d_geom);
+    carve(a.rec, g, gl.rec); carve(a.depth, g, gl.depth); carve(a.rect, g, gl.rect);
+    carve(a.clamped, g, gl.clamped); carve(a.acc, g, gl.acc); carve(a.vis_list, g, gl.vis_list);
+    char* im = align128(ws->d_image);
+    carve(a.final_T, im, il.final_T); carve(a.n_contrib, im, il.n_contrib); carve(a.last_entry, im, il.last_entry);
+    carve(a.ranges, im, il.ranges); carve(a.tile_count, im, il.tile_count); carve(a.cursor, im, il.cursor);
+    carve(a.list_tiny, im, il.list_tiny); carve(a.list_small, im, il.list_small);
+    carve(a.list_large, im, il.list_large); carve(a.list_huge, im, il.list_huge);
+    carve(a.tile_order, im, il.tile_order); carve(a.counters, im, il.counters);
+    char* bn = align128(ws->d_binning);      // NULL without a binning buffer
+    carve(a.point_list, bn, bl.point_list); carve(a.keys, bn, bl.keys); carve(a.keys_scratch, bn, bl.keys_scratch);
+    carve(a.sub_hits, bn, bl.sub_hits);
+    a.capacity = ws->binning_capacity;
+    a.status = ws->d_status;
     return FB200_OK;
 }
 
@@ -211,10 +249,6 @@ struct StageTimer {
         g_ev.recorded[stage] = true;
     }
 };
-
-inline char* align128(void* p) {
-    return reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(p) + 127) & ~uintptr_t(127));
-}
 
 }  // namespace
 
@@ -289,47 +323,10 @@ int fb200_get_layout(int32_t P, int32_t W, int32_t H, int64_t capacity, fb200_la
 
 static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws, bool need_binning,
                      float* d_out_color, int32_t* d_radii, FwdArgs& a) {
-    int rc = validate(prm, in, ws);
+    int rc = carve_frame(prm, in, ws, a);
     if (rc != FB200_OK) return rc;
     if (prm->P > 0 && !d_radii) return fail(FB200_EINVAL, "output pointers missing");
     if (need_binning && !d_out_color) return fail(FB200_EINVAL, "output pointers missing");
-    const GeomLayout gl((size_t)prm->P);
-    const ImageLayout il(prm->image_width, prm->image_height);
-    const BinLayout bl((size_t)ws->binning_capacity);
-    char* g = align128(ws->d_geom);
-    char* im = align128(ws->d_image);
-    char* bn = ws->d_binning ? align128(ws->d_binning) : nullptr;
-    memset(&a, 0, sizeof(a));
-    a.prm = *prm;
-    a.in = *in;
-    if (in->frosting) { a.frosting = 1; a.fr = *in->frosting; a.in = frosting_inputs(in); }
-    // focal lengths exactly as rasterizer_impl.cu:222-223
-    a.focal_y = prm->image_height / (2.0f * prm->tanfovy);
-    a.focal_x = prm->image_width / (2.0f * prm->tanfovx);
-    a.tiles_x = il.tiles_x; a.tiles_y = il.tiles_y;
-    a.rec = reinterpret_cast<SplatRec*>(g + gl.rec);
-    a.depth = reinterpret_cast<float*>(g + gl.depth);
-    a.rect = reinterpret_cast<uint2*>(g + gl.rect);
-    a.clamped = reinterpret_cast<uint8_t*>(g + gl.clamped);
-    a.vis_list = reinterpret_cast<uint32_t*>(g + gl.vis_list);
-    a.final_T = reinterpret_cast<float*>(im + il.final_T);
-    a.n_contrib = reinterpret_cast<uint32_t*>(im + il.n_contrib);
-    a.last_entry = reinterpret_cast<uint32_t*>(im + il.last_entry);
-    a.ranges = reinterpret_cast<uint2*>(im + il.ranges);
-    a.tile_count = reinterpret_cast<uint32_t*>(im + il.tile_count);
-    a.cursor = reinterpret_cast<uint32_t*>(im + il.cursor);
-    a.list_tiny = reinterpret_cast<uint32_t*>(im + il.list_tiny);
-    a.list_small = reinterpret_cast<uint32_t*>(im + il.list_small);
-    a.list_large = reinterpret_cast<uint32_t*>(im + il.list_large);
-    a.list_huge = reinterpret_cast<uint32_t*>(im + il.list_huge);
-    a.tile_order = reinterpret_cast<uint32_t*>(im + il.tile_order);
-    a.counters = reinterpret_cast<uint32_t*>(im + il.counters);
-    a.point_list = bn ? reinterpret_cast<uint32_t*>(bn + bl.point_list) : nullptr;
-    a.keys = bn ? reinterpret_cast<unsigned long long*>(bn + bl.keys) : nullptr;
-    a.keys_scratch = bn ? reinterpret_cast<unsigned long long*>(bn + bl.keys_scratch) : nullptr;
-    a.sub_hits = bn ? reinterpret_cast<uint32_t*>(bn + bl.sub_hits) : nullptr;
-    a.capacity = ws->binning_capacity;
-    a.status = ws->d_status;
     a.out_color = d_out_color;
     a.radii = d_radii;
     return FB200_OK;
@@ -337,7 +334,7 @@ static int setup_fwd(const fb200_params* prm, const fb200_inputs* in, const fb20
 
 int fb200_forward_geometry(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
                            int32_t* d_radii, void* stream) {
-    FwdArgs a;
+    FwdArgs a{};
     int rc = setup_fwd(prm, in, ws, false, nullptr, d_radii, a);
     if (rc != FB200_OK) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -347,9 +344,7 @@ int fb200_forward_geometry(const fb200_params* prm, const fb200_inputs* in, cons
       if ((rc = stage(launch_tile_scan(a, s), "tile scan", debug, s)) != FB200_OK) return rc; }
     if (ws->acc_zeroed_by_forward && prm->P > 0) {
         // backward's accumulators: cleared here, in the shadow of the host's wait for the instance count
-        const GeomLayout gl((size_t)prm->P);
-        float* acc = reinterpret_cast<float*>(align128(ws->d_geom) + gl.acc);
-        if ((rc = stage(cudaMemsetAsync(acc, 0, sizeof(float) * 12 * (size_t)prm->P, s), "accumulator clear", debug, s)) != FB200_OK)
+        if ((rc = stage(cudaMemsetAsync(a.acc, 0, sizeof(float) * 12 * (size_t)prm->P, s), "accumulator clear", debug, s)) != FB200_OK)
             return rc;
     }
     return FB200_OK;
@@ -357,7 +352,7 @@ int fb200_forward_geometry(const fb200_params* prm, const fb200_inputs* in, cons
 
 int fb200_forward_raster(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
                          float* d_out_color, int32_t* d_radii, void* stream) {
-    FwdArgs a;
+    FwdArgs a{};
     int rc = setup_fwd(prm, in, ws, true, d_out_color, d_radii, a);
     if (rc != FB200_OK) return rc;
     if ((rc = setup_extra(prm, true, false, a.ex)) != FB200_OK) return rc;
@@ -382,7 +377,8 @@ int fb200_forward(const fb200_params* prm, const fb200_inputs* in, const fb200_w
 
 int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_workspace* ws,
                    const int32_t* d_radii, const float* d_dL_dout_color, const fb200_grads* grads, void* stream) {
-    int rc = validate(prm, in, ws);
+    BwdArgs a{};
+    int rc = carve_frame(prm, in, ws, a);
     if (rc != FB200_OK) return rc;
     if (!grads || !d_dL_dout_color || (prm->P > 0 && !d_radii)) return fail(FB200_EINVAL, "backward pointers missing");
     // outputs a caller cannot use may be NULL and are then not written: dL/dcolors on the SH path (an intermediate
@@ -403,31 +399,7 @@ int fb200_backward(const fb200_params* prm, const fb200_inputs* in, const fb200_
     const bool debug = (prm->debug & 1) != 0;
     if (prm->P == 0) return FB200_OK;
 
-    const GeomLayout gl((size_t)prm->P);
-    const ImageLayout il(prm->image_width, prm->image_height);
-    const BinLayout bl((size_t)ws->binning_capacity);
-    char* g = align128(ws->d_geom);
-    char* im = align128(ws->d_image);
-    char* bn = ws->d_binning ? align128(ws->d_binning) : nullptr;
-
-    BwdArgs a;
-    memset(&a, 0, sizeof(a));
-    a.prm = *prm;
-    a.in = *in;
-    if (in->frosting) { a.frosting = 1; a.fr = *in->frosting; a.fg = *fg; a.in = frosting_inputs(in); }
-    a.focal_y = prm->image_height / (2.0f * prm->tanfovy);
-    a.focal_x = prm->image_width / (2.0f * prm->tanfovx);
-    a.tiles_x = il.tiles_x; a.tiles_y = il.tiles_y;
-    a.rec = reinterpret_cast<const SplatRec*>(g + gl.rec);
-    a.clamped = reinterpret_cast<const uint8_t*>(g + gl.clamped);
-    a.vis_list = reinterpret_cast<const uint32_t*>(g + gl.vis_list);
-    a.acc = reinterpret_cast<float*>(g + gl.acc);
-    a.final_T = reinterpret_cast<const float*>(im + il.final_T);
-    a.last_entry = reinterpret_cast<const uint32_t*>(im + il.last_entry);
-    a.tile_order = reinterpret_cast<const uint32_t*>(im + il.tile_order);
-    a.ranges = reinterpret_cast<const uint2*>(im + il.ranges);
-    a.sub_hits = bn ? reinterpret_cast<const uint32_t*>(bn + bl.sub_hits) : nullptr;
-    a.status = ws->d_status;
+    if (in->frosting) a.fg = *fg;
     a.radii = d_radii;
     a.dL_dpix = d_dL_dout_color;
     a.g = *grads;

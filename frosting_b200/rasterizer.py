@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._lib import Params, Inputs, Workspace, Grads, Layout, ptr
+from ._lib import Params, Inputs, Workspace, Grads, ptr
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -491,12 +491,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         # alpha = 1 - final_T: the reference computes and keeps final_T (forward.cu:369, imgBuffer) but never returns it
         alpha = color.new_empty(0)
         if return_alpha:
-            H, W = int(raster_settings.image_height), int(raster_settings.image_width)
-            lay = Layout()
-            _lib.check(_lib.lib().fb200_get_layout(call.prm.P, W, H, 0, C.byref(lay)))
-            base = (-call.image.data_ptr()) % 128
-            final_T = call.image[base + lay.img_final_T: base + lay.img_final_T + W * H * 4].view(torch.float32).view(H, W)
-            alpha = 1.0 - final_T
+            prm = call.prm
+            alpha = 1.0 - _lib.workspace_views(None, call.image, None, prm.P, prm.image_width, prm.image_height, 0,
+                                               0)["final_T"]
         ctx.mark_non_differentiable(alpha)
         return color, radii, extra, alpha
 
@@ -605,30 +602,12 @@ def forward_with_state(raster_settings, means3D, opacities, shs=None, colors_pre
             means3D, e if shs is None else shs, e if colors_precomp is None else colors_precomp, opacities,
             e if scales is None else scales, e if rotations is None else rotations,
             e if cov3D_precomp is None else cov3D_precomp, raster_settings, visibility_mask, exact=True)
-    P, W, H = call.prm.P, call.prm.image_width, call.prm.image_height
-    lay = Layout()
-    _lib.check(_lib.lib().fb200_get_layout(P, W, H, call.capacity, C.byref(lay)))
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    R = call.num_rendered
-
-    def view(buf, off, nbytes, dtype):
-        base = (-buf.data_ptr()) % 128   # the library aligns the base to 128 bytes
-        return buf[base + off: base + off + nbytes].view(dtype)
-
-    st = dict(
-        color=color, radii=radii, num_rendered=R, call=call,
-        rec=view(call.geom, lay.geom_rec, P * 48, torch.float32).view(P, 12),
-        depth=view(call.geom, lay.geom_depth, P * 4, torch.float32),
-        rect=view(call.geom, lay.geom_rect, P * 8, torch.int32).view(P, 2),
-        clamped=view(call.geom, lay.geom_clamped, P, torch.uint8),
-        final_T=view(call.image, lay.img_final_T, W * H * 4, torch.float32).view(H, W),
-        n_contrib=view(call.image, lay.img_n_contrib, W * H * 4, torch.int32).view(H, W),
-        ranges=view(call.image, lay.img_ranges, T * 8, torch.int32).view(T, 2),
-        tile_count=view(call.image, lay.img_tile_count, T * 4, torch.int32),
-        point_list=view(call.binning, lay.bin_point_list, R * 4, torch.int32),
-        keys=view(call.binning, lay.bin_keys, R * 8, torch.int64),
-    )
-    return st
+    prm, R = call.prm, call.num_rendered
+    v = _lib.workspace_views(call.geom, call.image, call.binning, prm.P, prm.image_width, prm.image_height,
+                             call.capacity, R)
+    return dict(color=color, radii=radii, num_rendered=R, call=call,
+                **{k: v[k] for k in ("rec", "depth", "rect", "clamped", "final_T", "n_contrib", "ranges", "tile_count",
+                                     "point_list", "keys")})
 
 
 def geometry_state(raster_settings, means3D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
@@ -641,17 +620,7 @@ def geometry_state(raster_settings, means3D, opacities, shs=None, colors_precomp
             means3D, e if shs is None else shs, e if colors_precomp is None else colors_precomp, opacities,
             e if scales is None else scales, e if rotations is None else rotations,
             e if cov3D_precomp is None else cov3D_precomp, raster_settings, visibility_mask, geometry_only=True)
-    P, W, H = call.prm.P, call.prm.image_width, call.prm.image_height
-    lay = Layout()
-    _lib.check(_lib.lib().fb200_get_layout(P, W, H, 0, C.byref(lay)))
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-
-    def view(buf, off, nbytes, dtype):
-        base = (-buf.data_ptr()) % 128
-        return buf[base + off: base + off + nbytes].view(dtype)
-
+    prm = call.prm
+    v = _lib.workspace_views(call.geom, call.image, None, prm.P, prm.image_width, prm.image_height, 0, 0)
     return dict(radii=radii, num_rendered=call.num_rendered, call=call,
-                depth=view(call.geom, lay.geom_depth, P * 4, torch.float32),
-                rect=view(call.geom, lay.geom_rect, P * 8, torch.int32).view(P, 2),
-                rec=view(call.geom, lay.geom_rec, P * 48, torch.float32).view(P, 12),
-                tile_count=view(call.image, lay.img_tile_count, T * 4, torch.int32))
+                **{k: v[k] for k in ("depth", "rect", "rec", "tile_count")})

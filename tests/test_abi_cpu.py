@@ -110,6 +110,31 @@ def test_layout_offsets_are_aligned_and_ordered():
     assert lay.bin_sub_hits + 4 * 8 * 5000 <= L.fb200_binning_bytes(5000)
 
 
+def test_workspace_views_start_at_the_aligned_base():
+    """_lib.workspace_views reads each sub-array where the library carves it: at its fb200_layout offset from the
+    buffer's first 128-byte aligned byte, whatever the buffer's own alignment."""
+    import torch
+    P, W, H, cap, R = 1000, 250, 130, 5000, 4000
+    L = _lib.lib()
+    lay = _lib.Layout()
+    assert L.fb200_get_layout(P, W, H, cap, C.byref(lay)) == 0
+    sizes = (L.fb200_geom_bytes(P), L.fb200_image_bytes(W, H), L.fb200_binning_bytes(cap))
+    bufs = [torch.zeros(n + 128, dtype=torch.uint8)[40:40 + n] for n in sizes]      # 8 bytes past a 64-byte boundary
+    assert all(b.data_ptr() % 128 for b in bufs)
+    g, im, bn = ((b.data_ptr() + 127) // 128 * 128 for b in bufs)
+    v = _lib.workspace_views(*bufs, P, W, H, cap, R)
+    T = 16 * 9
+    expect = dict(rec=(g + lay.geom_rec, (P, 12)), clamped=(g + lay.geom_clamped, (P,)), acc=(g + lay.geom_acc, (P, 12)),
+                  final_T=(im + lay.img_final_T, (H, W)), ranges=(im + lay.img_ranges, (T, 2)),
+                  tile_count=(im + lay.img_tile_count, (T,)), keys=(bn + lay.bin_keys, (R,)),
+                  sub_hits=(bn + lay.bin_sub_hits, (8 * R,)))
+    assert {k: (v[k].data_ptr(), tuple(v[k].shape)) for k in expect} == expect
+    assert v.keys() == {"rec", "depth", "rect", "clamped", "acc", "final_T", "n_contrib", "last_entry", "ranges",
+                        "tile_count", "point_list", "keys", "sub_hits"}
+    assert _lib.workspace_views(None, bufs[1], None, P, W, H, 0, 0).keys() == \
+        {"final_T", "n_contrib", "last_entry", "ranges", "tile_count"}
+
+
 def test_argument_errors_are_reported_without_touching_cuda():
     L = _lib.lib()
     lay = _lib.Layout()

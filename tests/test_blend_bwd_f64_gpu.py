@@ -28,7 +28,7 @@ import pytest
 import torch
 
 from frosting_b200 import _lib, scenes
-from frosting_b200._lib import Extra, Grads, Inputs, Layout, Params, Workspace
+from frosting_b200._lib import Extra, Grads, Inputs, Params, Workspace
 from oracle import blend_f64
 from tests.util import blend_regime_gaussians
 
@@ -45,10 +45,6 @@ EX_BG = (0.7, -1.3, 0.25)
 
 def _p(t):
     return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _u32(buf, off, n):
-    return buf[off:off + 4 * n].view(torch.int32).long()
 
 
 def _run(cam, g, ch, seed, dev):
@@ -97,25 +93,21 @@ def _run(cam, g, ch, seed, dev):
     grads = Grads(d_dL_dmeans2D=_p(out["means2D"]), d_dL_dcolors=_p(out["colors"]), d_dL_dopacity=_p(out["opacities"]),
                   d_dL_dmeans3D=_p(out["means3D"]), d_dL_dscales=_p(out["scales"]),
                   d_dL_drotations=_p(out["rotations"]), sparse_rows=0)
-    lay = Layout()
-    _lib.check(L.fb200_get_layout(P, W, H, R, C.byref(lay)))
+    v = _lib.workspace_views(geom, image, binning, P, W, H, R, R)
     accs, dfeats = [], []
     for zeroed in (1, 0):
         ws.acc_zeroed_by_forward = zeroed
         _lib.check(L.fb200_backward(C.byref(prm), C.byref(inp), C.byref(ws), _p(radii), _p(dpix), C.byref(grads),
                                     stream))
         torch.cuda.synchronize(dev)
-        accs.append(geom[lay.geom_acc:lay.geom_acc + 48 * P].view(torch.float32).view(P, 12).clone())
+        accs.append(v["acc"].clone())
         if ch:
             dfeats.append(ex["dfeat"].clone())
     assert int(status[_lib.ST_OVERFLOW]) == 0
-    T = ((W + 15) // 16) * ((H + 15) // 16)
     return dict(P=P, R=R, radii=radii, accs=accs, dfeats=dfeats, color=color, dpix=dpix, ex=ex,
-                rec=geom[lay.geom_rec:lay.geom_rec + 48 * P].view(torch.float32).view(P, 12).clone(),
-                final_T=image[lay.img_final_T:lay.img_final_T + 4 * H * W].view(torch.float32).clone(),
-                n_contrib=_u32(image, lay.img_n_contrib, H * W), last_entry=_u32(image, lay.img_last_entry, H * W),
-                ranges=_u32(image, lay.img_ranges, 2 * T).view(T, 2), point_list=_u32(binning, lay.bin_point_list, R),
-                sub_hits=_u32(binning, lay.bin_sub_hits, 8 * R))
+                rec=v["rec"].clone(), final_T=v["final_T"].flatten().clone(), n_contrib=v["n_contrib"].flatten().long(),
+                last_entry=v["last_entry"].flatten().long(), ranges=v["ranges"].long(),
+                point_list=v["point_list"].long(), sub_hits=v["sub_hits"].long())
 
 
 def _subtiles(dev):

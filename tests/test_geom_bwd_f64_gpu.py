@@ -26,7 +26,7 @@ import torch
 
 import frosting_b200 as fb
 from frosting_b200 import _lib, scenes
-from frosting_b200._lib import Grads, Inputs, Layout, Params, Workspace
+from frosting_b200._lib import Grads, Inputs, Params, Workspace
 from frosting_b200.frosting_render import BG_KEYS, MESH_KEYS, FrostingBlock
 from oracle import geom_f64
 from tests.util import regime_gaussians
@@ -72,10 +72,9 @@ def _run(rs, P, M, D, inp, grads, dev):
     cot = torch.randn(3, H, W, generator=torch.Generator().manual_seed(P % 97)).to(dev)
     _lib.check(L.fb200_backward(C.byref(prm), C.byref(inp), C.byref(ws), _p(radii), _p(cot), C.byref(grads), stream))
     torch.cuda.synchronize(dev)
-    lay = Layout()
-    _lib.check(L.fb200_get_layout(P, W, H, R, C.byref(lay)))
-    acc = geom[lay.geom_acc:lay.geom_acc + 48 * P].view(torch.float32).view(P, 12).clone()
-    bits = geom[lay.geom_clamped:lay.geom_clamped + P].clone()
+    v = _lib.workspace_views(geom, image, binning, P, W, H, R, R)
+    acc = v["acc"].clone()
+    bits = v["clamped"].clone()
     clamped = torch.stack([(bits >> c) & 1 for c in range(3)], 1).bool()
     assert int(status[_lib.ST_OVERFLOW]) == 0
     return radii, acc, clamped
