@@ -14,7 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libfrosting_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "geom_bwd.cu", "mesh_vis.cu",
-           "frosting_attr.cu", "frosting_edit.cu", "frosting_skin.cu", "texture.cu", "loss.cu", "optim.cu", "sugar_reg.cu"]
+           "frosting_attr.cu", "frosting_edit.cu", "frosting_skin.cu", "texture.cu", "loss.cu", "optim.cu", "sugar_reg.cu",
+           "knn.cu"]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [

@@ -713,6 +713,32 @@ int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms,
                  "sugar_reg_backward");
 }
 
+size_t fb200_knn_workspace_bytes(int32_t P, int32_t Q, int32_t K) {
+    return (P >= 1 && Q >= 0 && K >= 1 && K <= 32 && K <= P) ? knn_workspace_bytes(P, Q) : 0;
+}
+
+int fb200_knn(const float* d_points, int32_t P, const float* d_queries, int32_t Q, int32_t K, void* d_workspace,
+              size_t workspace_bytes, float* d_dists, int64_t* d_idx, void* stream) {
+    if (P < 1 || Q < 0 || K < 1 || K > 32 || K > P)
+        return fail(FB200_EINVAL, "knn: bad extents (1 <= K <= 32, K <= P, Q >= 0)");
+    if (!d_queries && Q != P) return fail(FB200_EINVAL, "knn: self queries (no query pointer) need Q == P");
+    if (Q == 0) return FB200_OK;
+    if (!d_points || !d_workspace || !d_dists || !d_idx) return fail(FB200_EINVAL, "knn: missing pointer");
+    if (misaligned(d_workspace, 256)) return fail(FB200_EINVAL, "knn: the workspace must be 256-byte aligned");
+    if (workspace_bytes < knn_workspace_bytes(P, d_queries ? Q : 0)) return fail(FB200_ENOSPC, "knn: workspace too small");
+    size_t need, reserved;
+    int rc = check(knn_sort_scratch(P, d_queries ? Q : 0, &need, &reserved), "knn: radix-sort scratch query");
+    if (rc != FB200_OK) return rc;
+    if (need > reserved) {
+        char msg[160];
+        snprintf(msg, sizeof(msg), "knn: this CUB's radix sort needs %zu bytes of scratch, the workspace reserves %zu",
+                 need, reserved);
+        return fail(FB200_ENOSPC, msg);
+    }
+    return check(launch_knn(d_points, P, d_queries, Q, K, d_workspace, d_dists, d_idx, static_cast<cudaStream_t>(stream)),
+                 "knn");
+}
+
 int fb200_adam_step(const fb200_adam_args* a, void* stream) {
     if (!a) return fail(FB200_EINVAL, "adam_step: null args");
     if (a->world < 1 || a->world > FB200_MAX_PEERS || a->rank < 0 || a->rank >= a->world)

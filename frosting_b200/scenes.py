@@ -781,3 +781,60 @@ def sugar_scene(P, seed, K=16, straggler_frac=0.1, device="cpu"):
     knn = torch.from_numpy(cKDTree(points.double().numpy()).query(points.double().numpy(), k=K)[1]).long().reshape(P, K)
     to =lambda t: t.contiguous().to(device)
     return dict(points=to(points), scaling=to(scaling), quaternions=to(q), strengths=to(strengths), knn_idx=to(knn))
+
+
+# ---- point sets for the exact K-nearest-neighbour search (knn.py) ----
+
+KNN_SCENES = ("sugar", "cube", "plane", "line", "lattice", "coincident", "offset")
+
+
+def knn_scene(kind, P, seed, outlier_frac=0.01):
+    """float32 [P,3] point sets (CPU) for knn_points:
+      sugar       a SuGaR-like coarse scene: centres on the bumpy sphere of `sugar_scene`, 10 % scattered within 0.3
+                  of it, and `outlier_frac` far background Gaussians at 10 to 10^4 surface spacings beyond it
+      cube        uniform in the unit cube
+      plane       uniform in a square, z constant
+      line        uniform on a segment
+      lattice     the integer lattice n^3 (P = n^3), in a random order: most distances tie exactly
+      coincident  min(5000, P // 2) copies of one point, the rest pairs of clones, in a random order
+      offset      a small sphere near (1000, 1000, 1000) with spacing ~1e-3: distances near the float32 rounding
+    """
+    g = torch.Generator().manual_seed(seed)
+    if kind == "sugar":
+        d = torch.nn.functional.normalize(torch.randn(P, 3, generator=g), dim=-1)
+        bump = 1.0 + 0.08 * torch.sin(5 * d[:, 0]) * torch.cos(4 * d[:, 1])
+        pts = torch.tensor([0.0, 0.0, 6.0]) + 2.0 * bump[:, None] * d
+        spacing = math.sqrt(4 * math.pi * 4.0 / max(P, 1))
+        n_far = int(outlier_frac * P)
+        n_near = int(0.1 * P)
+        pts[P - n_near - n_far:P - n_far] += 0.3 * torch.randn(n_near, 3, generator=g)
+        far = torch.nn.functional.normalize(torch.randn(n_far, 3, generator=g), dim=-1)
+        dist = 2.0 + spacing * 10.0 ** (1 + 3 * torch.rand(n_far, 1, generator=g))
+        pts[P - n_far:] = torch.tensor([0.0, 0.0, 6.0]) + dist * far
+        return pts[torch.randperm(P, generator=g)].contiguous()
+    if kind == "cube":
+        return torch.rand(P, 3, generator=g)
+    if kind == "plane":
+        pts = torch.rand(P, 3, generator=g)
+        pts[:, 2] = 0.25
+        return pts
+    if kind == "line":
+        t = torch.rand(P, 1, generator=g)
+        return (torch.tensor([0.1, -0.2, 3.0]) + t * torch.tensor([1.0, 0.5, -0.25])).contiguous()
+    if kind == "lattice":
+        n = round(P ** (1 / 3))
+        if n ** 3 != P:
+            raise ValueError(f"a lattice needs a cube P, got {P}")
+        a = torch.arange(n, dtype=torch.float32)
+        pts = torch.stack(torch.meshgrid(a, a, a, indexing="ij"), -1).reshape(P, 3)
+        return pts[torch.randperm(P, generator=g)].contiguous()
+    if kind == "coincident":
+        m = min(5000, P // 2)
+        pairs = torch.rand((P - m + 1) // 2, 3, generator=g).repeat_interleave(2, 0)[:P - m]
+        pts = torch.cat([torch.full((m, 3), 0.5), pairs])
+        return pts[torch.randperm(P, generator=g)].contiguous()
+    if kind == "offset":
+        r = 1e-3 * math.sqrt(P / (4 * math.pi))
+        d = torch.nn.functional.normalize(torch.randn(P, 3, generator=g), dim=-1)
+        return (torch.tensor([1000.0, 1000.0, 1000.0]) + r * d).contiguous()
+    raise ValueError(f"unknown knn scene {kind!r}; one of {KNN_SCENES}")

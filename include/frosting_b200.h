@@ -465,6 +465,23 @@ int fb200_sugar_reg_forward(const fb200_sugar_reg* r, int32_t with_grad, float* 
 int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms, float* d_dpoints, float* d_dscaling,
                              float* d_dquaternions, float* d_dstrengths, void* stream);
 
+/* Exact K nearest neighbours (pytorch3d's knn_points(queries[None], points[None], K).dists[0] / .idx[0] with norm = 2;
+ * SuGaR's neighbour table, frosting_scene/sugar_model.py:249, :1044-1061).  For each query q, d_dists [Q,K] and d_idx
+ * [Q,K] hold the first K points p in ascending (d, index) order, compared lexicographically, where
+ *   d = fmaf(dz, dz, fmaf(dy, dy, dx * dx)),  dx = q.x - p.x rounded to float32 (likewise y, z),
+ * so the result is a function of the input bits alone: on distinct points a self query lists the point itself first
+ * (d = 0), and ties go to the lower index.  d_queries NULL: the points themselves, Q == P.  Extents 1 <= K <= 32, K <= P,
+ * Q >= 0 (Q = 0: nothing is launched); P and Q are int32, so below 2^31.  Point and query rows are [n,3] float32.
+ * The inputs are specified for finite coordinates only; given any bits the call still terminates and writes indices in
+ * [0, P), and the first int32 of the workspace becomes nonzero (stream-ordered) when a point or query coordinate is not
+ * finite.  Stream-ordered on `stream`, no host synchronisation, no allocation.  The workspace is 256-byte aligned and
+ * fb200_knn_workspace_bytes(P, Q, K) bytes for Q separate queries, (P, 0, K) for self queries: at most 48 bytes per
+ * point plus 48 per separate query plus 72 KiB (0 for bad extents; host only, no CUDA call).  A shorter workspace is
+ * FB200_ENOSPC. */
+size_t fb200_knn_workspace_bytes(int32_t P, int32_t Q, int32_t K);
+int fb200_knn(const float* d_points, int32_t P, const float* d_queries, int32_t Q, int32_t K, void* d_workspace,
+              size_t workspace_bytes, float* d_dists, int64_t* d_idx, void* stream);
+
 /* Data-parallel gradient reduction fused with the Adam update (SURVEY.md row f3).  Replaces "all-reduce every
  * .grad, then torch.optim.Adam(l, lr=0.0, eps=1e-15).step()" (frosting_scene/frosting_optimizer.py:101,116-118) for
  * camera-sharded training.  All learnable tensors of a rank live in ONE flat fp32 parameter slab and their gradients
