@@ -12,6 +12,7 @@ from .skin import FrostingSkin, skin_tables
 from .texture import TextureBaker, compute_textured_mesh, mesh_bary, write_textured_obj
 from .loss import l1_dssim_loss
 from .sugar import SugarNeighbours, sample_in_gaussians, sdf_regularization
+from .sugar_dn import depth_normal_consistency, depth_normal_features
 from .knn import KNN, knn_points
 from .optim import FrostingAdam, OptimizationParams
 from .mesh import (MeshRasterizer, RasterizationSettings, Fragments, nvdiff_rasterization,
@@ -21,7 +22,7 @@ __all__ = [
     "GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "forward_with_state",
     "MeshRasterizer", "RasterizationSettings", "Fragments", "nvdiff_rasterization",
     "nvdiff_rasterization_with_pix_to_face", "rasterize_mesh", "gaussian_render_mask",
-    "install_as_diff_gaussian_rasterization", "frosting_attributes_fused", "frosting_render", "frosting_render_two_step", "FrostingEdit", "FrostingEditComplex", "frosting_render_edited", "FrostingSkin", "skin_tables", "TextureBaker", "compute_textured_mesh", "mesh_bary", "write_textured_obj", "l1_dssim_loss", "SugarNeighbours", "sample_in_gaussians", "sdf_regularization", "KNN", "knn_points", "FrostingAdam", "OptimizationParams",
+    "install_as_diff_gaussian_rasterization", "frosting_attributes_fused", "frosting_render", "frosting_render_two_step", "FrostingEdit", "FrostingEditComplex", "frosting_render_edited", "FrostingSkin", "skin_tables", "TextureBaker", "compute_textured_mesh", "mesh_bary", "write_textured_obj", "l1_dssim_loss", "SugarNeighbours", "sample_in_gaussians", "sdf_regularization", "depth_normal_features", "depth_normal_consistency", "KNN", "knn_points", "FrostingAdam", "OptimizationParams",
 ]
 
 

@@ -209,6 +209,11 @@ SIGNATURES = {
     "fb200_sugar_reg_workspace_bytes": (_size, [_i32, _i32, _i32, _i32]),
     "fb200_sugar_reg_forward": (_int, [C.POINTER(SugarReg), _i32, _vp, _vp]),
     "fb200_sugar_reg_backward": (_int, [C.POINTER(SugarReg)] + [_vp] * 6),
+    "fb200_sugar_dn_features": (_int, [_i32] + [_vp] * 7),
+    "fb200_sugar_dn_features_backward": (_int, [_i32] + [_vp] * 9),
+    "fb200_sugar_dn_partials": (_size, [_i32, _i32]),
+    "fb200_sugar_dn_loss_forward": (_int, [_vp, _i32, _i32] + [_vp] * 5),
+    "fb200_sugar_dn_loss_backward": (_int, [_vp, _i32, _i32] + [_vp] * 5),
     "fb200_knn_workspace_bytes": (_size, [_i32, _i32, _i32]),
     "fb200_knn": (_int, [_vp, _i32, _vp, _i32, _i32, _vp, _size, _vp, _vp, _vp]),
     "fb200_adam_step": (_int, [C.POINTER(AdamArgs), _vp]),

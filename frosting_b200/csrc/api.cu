@@ -713,6 +713,67 @@ int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms,
                  "sugar_reg_backward");
 }
 
+static int check_sugar_dn_features(int32_t P, const float* d_points, const float* d_scaling, const float* d_quaternions,
+                                   const float* d_viewmatrix, const float* d_campos) {
+    if (P < 0) return fail(FB200_EINVAL, "sugar_dn_features: P must be >= 0");
+    if (P > 0 && (!d_points || !d_scaling || !d_quaternions || !d_viewmatrix || !d_campos))
+        return fail(FB200_EINVAL, "sugar_dn_features: missing input pointer");
+    if (misaligned(d_quaternions, 16)) return fail(FB200_EINVAL, "sugar_dn_features: quaternions must be 16-byte aligned");
+    return FB200_OK;
+}
+
+int fb200_sugar_dn_features(int32_t P, const float* d_points, const float* d_scaling, const float* d_quaternions,
+                            const float* d_viewmatrix, const float* d_campos, float* d_features, void* stream) {
+    int rc = check_sugar_dn_features(P, d_points, d_scaling, d_quaternions, d_viewmatrix, d_campos);
+    if (rc != FB200_OK) return rc;
+    if (P > 0 && !d_features) return fail(FB200_EINVAL, "sugar_dn_features: missing features output");
+    return check(launch_sugar_dn_features(P, d_points, d_scaling, d_quaternions, d_viewmatrix, d_campos, d_features,
+                                          static_cast<cudaStream_t>(stream)), "sugar_dn_features");
+}
+
+int fb200_sugar_dn_features_backward(int32_t P, const float* d_points, const float* d_scaling,
+                                     const float* d_quaternions, const float* d_viewmatrix, const float* d_campos,
+                                     const float* d_dL_dfeatures, float* d_dpoints, float* d_dquaternions,
+                                     void* stream) {
+    int rc = check_sugar_dn_features(P, d_points, d_scaling, d_quaternions, d_viewmatrix, d_campos);
+    if (rc != FB200_OK) return rc;
+    if (P > 0 && (!d_dL_dfeatures || !d_dpoints || !d_dquaternions))
+        return fail(FB200_EINVAL, "sugar_dn_features_backward: missing gradient pointer");
+    if (misaligned(d_dquaternions, 16))
+        return fail(FB200_EINVAL, "sugar_dn_features_backward: dL/dquaternions must be 16-byte aligned");
+    return check(launch_sugar_dn_features_bwd(P, d_points, d_scaling, d_quaternions, d_viewmatrix, d_campos,
+                                              d_dL_dfeatures, d_dpoints, d_dquaternions,
+                                              static_cast<cudaStream_t>(stream)),
+                 "sugar_dn_features_backward");
+}
+
+size_t fb200_sugar_dn_partials(int32_t H, int32_t W) { return (H > 0 && W > 0) ? sugar_dn_num_partials(H, W) : 0; }
+
+static int check_sugar_dn_loss(const float* d_dn, int32_t H, int32_t W, const float* d_viewmatrix,
+                               const float* d_projmatrix) {
+    if (H <= 0 || W <= 0) return fail(FB200_EINVAL, "sugar_dn_loss: bad image size (H, W > 0)");
+    if (!d_dn || !d_viewmatrix || !d_projmatrix) return fail(FB200_EINVAL, "sugar_dn_loss: missing input pointer");
+    return FB200_OK;
+}
+
+int fb200_sugar_dn_loss_forward(const float* d_dn, int32_t H, int32_t W, const float* d_viewmatrix,
+                                const float* d_projmatrix, float* d_partials, float* d_loss, void* stream) {
+    int rc = check_sugar_dn_loss(d_dn, H, W, d_viewmatrix, d_projmatrix);
+    if (rc != FB200_OK) return rc;
+    if (!d_partials || !d_loss) return fail(FB200_EINVAL, "sugar_dn_loss_forward: missing output pointer");
+    return check(launch_sugar_dn_loss_fwd(d_dn, H, W, d_viewmatrix, d_projmatrix, d_partials, d_loss,
+                                          static_cast<cudaStream_t>(stream)), "sugar_dn_loss_forward");
+}
+
+int fb200_sugar_dn_loss_backward(const float* d_dn, int32_t H, int32_t W, const float* d_viewmatrix,
+                                 const float* d_projmatrix, const float* d_dL_dloss, float* d_dL_ddn, void* stream) {
+    int rc = check_sugar_dn_loss(d_dn, H, W, d_viewmatrix, d_projmatrix);
+    if (rc != FB200_OK) return rc;
+    if (!d_dL_dloss || !d_dL_ddn) return fail(FB200_EINVAL, "sugar_dn_loss_backward: missing gradient pointer");
+    return check(launch_sugar_dn_loss_bwd(d_dn, H, W, d_viewmatrix, d_projmatrix, d_dL_dloss, d_dL_ddn,
+                                          static_cast<cudaStream_t>(stream)), "sugar_dn_loss_backward");
+}
+
 size_t fb200_knn_workspace_bytes(int32_t P, int32_t Q, int32_t K) {
     return (P >= 1 && Q >= 0 && K >= 1 && K <= 32 && K <= P) ? knn_workspace_bytes(P, Q) : 0;
 }

@@ -170,6 +170,12 @@ GaussW make_window() {
 
 }  // namespace
 
+cudaError_t launch_loss_reduce(const float* partials, int n, float scale, float* out, cudaStream_t s) {
+    loss_reduce_kernel<<<1, 1024, 0, s>>>(partials, n, scale, out);
+    count_launch();
+    return cudaGetLastError();
+}
+
 size_t l1_dssim_num_partials(int C, int H, int W) {
     return (size_t)C * ((H + kLossTile - 1) / kLossTile) * ((W + kLossTile - 1) / kLossTile);
 }
@@ -178,10 +184,8 @@ cudaError_t launch_l1_dssim_fwd(const float* pred, const float* gt, int C, int H
                                 float* partials, float* loss, cudaStream_t s) {
     const dim3 grid((W + kLossTile - 1) / kLossTile, (H + kLossTile - 1) / kLossTile, C), block(kLossTile, kLossTile);
     l1_dssim_fwd_kernel<<<grid, block, 0, s>>>(pred, gt, C, H, W, lambda, make_window(), maps, partials);
-    const int n = (int)l1_dssim_num_partials(C, H, W);
-    loss_reduce_kernel<<<1, 1024, 0, s>>>(partials, n, 1.0f / (float)((double)C * H * W), loss);
-    count_launch(2);
-    return cudaGetLastError();
+    count_launch();
+    return launch_loss_reduce(partials, (int)l1_dssim_num_partials(C, H, W), 1.0f / (float)((double)C * H * W), loss, s);
 }
 
 cudaError_t launch_l1_dssim_bwd(const float* pred, const float* gt, const float* maps, int C, int H, int W, float lambda,

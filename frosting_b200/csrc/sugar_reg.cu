@@ -24,6 +24,7 @@
 // inclusively, min / argmin route to the first minimal axis.  Accumulation order of the atomics is not fixed, so the
 // gradients are reproducible to float rounding only; the two terms are bit-reproducible.
 #include "common.cuh"
+#include "sugar_common.cuh"
 
 namespace fb200 {
 
@@ -45,25 +46,6 @@ enum : int {
     kAccQuat = 6,       // e: dq (w, x, y, z)           (owner, through the sample's rotation)
     kAccScale = 7,      // e: ds.xyz, -                 (owner, through the sample's scale)
 };
-
-// pytorch3d quaternion_to_matrix, row-major: R[3 r + c]
-__device__ __forceinline__ void quat_to_matrix(float r, float i, float j, float k, float R[9]) {
-    const float two_s = 2.0f / (r * r + i * i + j * j + k * k);
-    R[0] = 1.f - two_s * (j * j + k * k); R[1] = two_s * (i * j - k * r); R[2] = two_s * (i * k + j * r);
-    R[3] = two_s * (i * j + k * r); R[4] = 1.f - two_s * (i * i + k * k); R[5] = two_s * (j * k - i * r);
-    R[6] = two_s * (i * k - j * r); R[7] = two_s * (j * k + i * r); R[8] = 1.f - two_s * (i * i + j * j);
-}
-
-// torch.min(dim=-1): the first minimal axis
-__device__ __forceinline__ int argmin3(float a, float b, float c) {
-    int m = 0;
-    float v = a;
-    if (b < v) { m = 1; v = b; }
-    if (c < v) m = 2;
-    return m;
-}
-
-__device__ __forceinline__ float sign_of(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); }
 
 __global__ void __launch_bounds__(kThreads)
 sugar_record_kernel(int P, const float* __restrict__ points, const float* __restrict__ scaling,
@@ -349,22 +331,8 @@ sugar_chain_kernel(int P, int reps, const float* __restrict__ scaling, const flo
     dR[6 + c] += ge * a5.z + gn * a4.z;
     d_scaling[p3] = ds[0]; d_scaling[p3 + 1] = ds[1]; d_scaling[p3 + 2] = ds[2];
 
-    // quaternion_to_matrix backward, two_s = 2 / |q|^2 included
-    const float r = q.x, i = q.y, j = q.z, k = q.w;
-    const float two_s = 2.0f / (r * r + i * i + j * j + k * k);
-    const float dts = -dR[0] * (j * j + k * k) + dR[1] * (i * j - k * r) + dR[2] * (i * k + j * r) +
-                      dR[3] * (i * j + k * r) - dR[4] * (i * i + k * k) + dR[5] * (j * k - i * r) +
-                      dR[6] * (i * k - j * r) + dR[7] * (j * k + i * r) - dR[8] * (i * i + j * j);
-    const float dr_ = two_s * (-dR[1] * k + dR[2] * j + dR[3] * k - dR[5] * i - dR[6] * j + dR[7] * i);
-    const float di = two_s * (dR[1] * j + dR[2] * k + dR[3] * j - 2.f * dR[4] * i - dR[5] * r + dR[6] * k + dR[7] * r -
-                              2.f * dR[8] * i);
-    const float dj = two_s * (-2.f * dR[0] * j + dR[1] * i + dR[2] * r + dR[3] * i + dR[5] * k - dR[6] * r + dR[7] * k -
-                              2.f * dR[8] * j);
-    const float dk = two_s * (-2.f * dR[0] * k - dR[1] * r + dR[2] * i + dR[3] * r - 2.f * dR[4] * k + dR[5] * j +
-                              dR[6] * i + dR[7] * j);
-    const float rad = -two_s * two_s * dts;      // d(two_s)/dq = -two_s^2 q
-    d_quats[p] = make_float4(dr_ + rad * r + ge * a6.x, di + rad * i + ge * a6.y, dj + rad * j + ge * a6.z,
-                             dk + rad * k + ge * a6.w);
+    const float4 dq = quat_to_matrix_bwd(q.x, q.y, q.z, q.w, dR);
+    d_quats[p] = make_float4(dq.x + ge * a6.x, dq.y + ge * a6.y, dq.z + ge * a6.z, dq.w + ge * a6.w);
 }
 
 int group_width(int K) {

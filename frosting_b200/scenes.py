@@ -532,7 +532,7 @@ def deform_base(verts, t=1.0, centre=(0.0, 0.0, 6.0)):
 # (tests/golden/make_frosting_skin_golden.py) runs the reference's own source on top of it.
 
 class Transform3d:
-    """The slice of pytorch3d.transforms.Transform3d the reference's skinning uses."""
+    """The slice of pytorch3d.transforms.Transform3d the reference's skinning and SuGaR's depth-normal render use."""
 
     def __init__(self, dtype=torch.float32, device="cpu", matrix=None):
         self._matrix = torch.eye(4, dtype=dtype, device=device).view(1, 4, 4) if matrix is None else matrix.view(-1, 4, 4)
@@ -557,6 +557,12 @@ class Transform3d:
         if out.shape[0] == 1 and points.dim() == 2:
             out = out.reshape(points.shape)
         return out
+
+    def transform_normals(self, normals):
+        """normals @ inverse(M[:3,:3]^T): the inverse transpose of the linear part, as pytorch3d applies it."""
+        mat = self.get_matrix()[:, :3, :3]
+        out = (normals if normals.dim() == 3 else normals[None]).bmm(mat.transpose(1, 2).inverse())
+        return out.reshape(normals.shape) if normals.dim() == 2 else out
 
 
 def skin_vertices(package, ref_indices, i_frame, base_verts):

@@ -465,6 +465,38 @@ int fb200_sugar_reg_forward(const fb200_sugar_reg* r, int32_t with_grad, float* 
 int fb200_sugar_reg_backward(const fb200_sugar_reg* r, const float* d_dL_dterms, float* d_dpoints, float* d_dscaling,
                              float* d_dquaternions, float* d_dstrengths, void* stream);
 
+/* SuGaR's depth-normal consistency of the coarse `dn_consistency` trainer (SURVEY.md row 17;
+ * frosting_scene/sugar_model.py:2343-2387 render_depth_and_normal, frosting_trainers/coarse_density_and_dn_consistency.py
+ * :17-95 depth_normal_consistency_loss).  The camera is the rasterizer's own: d_viewmatrix is world_view_transform and
+ * d_projmatrix full_proj_transform (row-major [4,4], row-vector convention), d_campos the camera centre [3]; all stay on
+ * the device.
+ *
+ * Features, one row per Gaussian, to be blended as 3 extra channels (fb200_extra) with background 0:
+ *   n = the column of quaternion_to_matrix(q) (raw q, pytorch3d's two_s = 2/|q|^2) at the first minimal axis of s,
+ *   n *= sign(n . (campos - p)) (0 gives a zero normal), features = {z, -(V n).x, -(V n).y} with V the COLMAP view
+ *   rotation: z and the normal's x, y in pytorch3d's view frame, diag(-1, -1, 1) times the COLMAP one.
+ * d_points, d_scaling, d_features [P,3]; d_quaternions [P,4] (w, x, y, z), 16-byte aligned.  The backward writes
+ * dL/dpoints (through z only) and dL/dquaternions (16-byte aligned) from dL/dfeatures; dL/dscaling is zero (argmin is
+ * discrete) and not written.
+ *
+ * Loss over the blended image d_dn [3,H,W]: depth dn[0], normal (-dn[1], -dn[2], -sqrt(1 - min(dn[1]^2 + dn[2]^2, 1)));
+ * points d ray(x, y) at integer pixel coordinates, ray = c2w[:3,:3] K^-1 (x, y, 1) as depths_to_points derives it;
+ * at interior pixels n_d = normalize(cross(P[r+1,c] - P[r-1,c], P[r,c+1] - P[r,c-1])) (eps 1e-12), 0 at border pixels;
+ * d_loss[0] = mean over the H W pixels of 1 - normal . (n_d @ V[:3,:3]).  d_partials [fb200_sugar_dn_partials(H, W)].
+ * The backward writes d_dL_ddn [3,H,W] (every element), scaled by the device scalar d_dL_dloss[0], without atomics.
+ * H < 3 or W < 3: every pixel is a border pixel, the loss is 1 and the gradient 0, and no kernel is launched. */
+int fb200_sugar_dn_features(int32_t P, const float* d_points, const float* d_scaling, const float* d_quaternions,
+                            const float* d_viewmatrix, const float* d_campos, float* d_features, void* stream);
+int fb200_sugar_dn_features_backward(int32_t P, const float* d_points, const float* d_scaling,
+                                     const float* d_quaternions, const float* d_viewmatrix, const float* d_campos,
+                                     const float* d_dL_dfeatures, float* d_dpoints, float* d_dquaternions,
+                                     void* stream);
+size_t fb200_sugar_dn_partials(int32_t H, int32_t W);
+int fb200_sugar_dn_loss_forward(const float* d_dn, int32_t H, int32_t W, const float* d_viewmatrix,
+                                const float* d_projmatrix, float* d_partials, float* d_loss, void* stream);
+int fb200_sugar_dn_loss_backward(const float* d_dn, int32_t H, int32_t W, const float* d_viewmatrix,
+                                 const float* d_projmatrix, const float* d_dL_dloss, float* d_dL_ddn, void* stream);
+
 /* Exact K nearest neighbours (pytorch3d's knn_points(queries[None], points[None], K).dists[0] / .idx[0] with norm = 2;
  * SuGaR's neighbour table, frosting_scene/sugar_model.py:249, :1044-1061).  For each query q, d_dists [Q,K] and d_idx
  * [Q,K] hold the first K points p in ascending (d, index) order, compared lexicographically, where
