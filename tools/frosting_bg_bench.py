@@ -15,7 +15,6 @@ attributes differ by an ulp).  Prints the card and its power limit with the numb
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -24,15 +23,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import frosting_b200 as fb                       # noqa: E402
 from frosting_b200 import scenes                 # noqa: E402
 from frosting_b200.frosting_render import BG_KEYS, MESH_KEYS   # noqa: E402
-
-
-def power_limit():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=20)
-        return r.stdout.strip() or "unknown"
-    except Exception:
-        return "unknown"
+from tools import timing                                       # noqa: E402
 
 
 def main():
@@ -47,7 +38,8 @@ def main():
     cam0 = scenes.make_camera(W, H)
     cam = scenes.ring_cameras(8, W, H, radius=6.0, device=dev)[0]
     rs = scenes.settings_for(cam, 3, device=dev)
-    result = {"gpu": torch.cuda.get_device_name(dev), "power_limit": power_limit(), "n_mesh": args.n_mesh, "runs": []}
+    gpu = timing.card()
+    result = {"card": gpu, "gpu": gpu["name"], "power_limit": gpu["power_limit"], "n_mesh": args.n_mesh, "runs": []}
     for n_bg in args.n_bg:
         params, mesh = scenes.frosting_layer(args.n_mesh, cam0, 1237, n_faces_target=max(1000, args.n_mesh // 2),
                                              n_background=n_bg)
@@ -73,24 +65,12 @@ def main():
             (color * cot).sum().backward()
             return color, radii
 
-        routes = {"a_frosting_render": route_a, "b_torch_cat_rasterizer": route_b}
-        outs = {}
-        for name, fn in routes.items():
-            for _ in range(args.warmup):
-                for p in params.values():
-                    p.grad = None
-                outs[name] = fn()
-        times = {name: [] for name in routes}
-        for _ in range(args.iters):
-            for name, fn in routes.items():
-                for p in params.values():
-                    p.grad = None
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                fn()
-                e1.record()
-                e1.synchronize()
-                times[name].append(e0.elapsed_time(e1))
+        def clear_grads():
+            for p in params.values():
+                p.grad = None
+
+        times, outs = timing.alternate({"a_frosting_render": route_a, "b_torch_cat_rasterizer": route_b}, args.iters,
+                                       args.warmup, before=clear_grads)
         (ca, ra), (cb, rb) = outs["a_frosting_render"], outs["b_torch_cat_rasterizer"]
         d = (ca - cb).abs()
         check = {"radii_mismatch_frac": (ra != rb).float().mean().item(),
@@ -98,16 +78,13 @@ def main():
         check["ok"] = check["radii_mismatch_frac"] < 1e-3 and check["image_px_over_1e-4_frac"] < 1e-3 and \
             check["image_max_abs_diff"] < 2e-2
         run = {"n_bg": n_bg, "rendered": int((ra > 0).sum()), "rendered_bg": int((ra[args.n_mesh:] > 0).sum()),
-               "check": check}
-        for name, t in times.items():
-            t = sorted(t)
-            run[name] = {"median_ms": t[len(t) // 2], "min_ms": t[0], "max_ms": t[-1]}
+               "check": check, **times}
         run["speedup_b_over_a"] = run["b_torch_cat_rasterizer"]["median_ms"] / run["a_frosting_render"]["median_ms"]
         result["runs"].append(run)
         print(json.dumps(run), flush=True)
         del params, mesh, outs
         torch.cuda.empty_cache()
-    print(json.dumps(result))
+    timing.emit(result)
 
 
 if __name__ == "__main__":

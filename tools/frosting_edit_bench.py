@@ -22,9 +22,9 @@ Reports the median of `--iters` frames per route, the max image difference and r
 and the card and its power limit.
 """
 import argparse
+import itertools
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -33,15 +33,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import frosting_b200 as fb                       # noqa: E402
 from frosting_b200 import rasterizer as R        # noqa: E402
 from frosting_b200 import scenes                 # noqa: E402
-
-
-def power_limit():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=20)
-        return r.stdout.strip() or "unknown"
-    except Exception:
-        return "unknown"
+from tools import timing                         # noqa: E402
 
 
 def main():
@@ -58,7 +50,8 @@ def main():
     W, H = 1920, 1080
     cam = scenes.ring_cameras(8, W, H, radius=6.0, device=dev)[0]
     rs = scenes.settings_for(cam, 3, device=dev)
-    result = {"gpu": torch.cuda.get_device_name(dev), "power_limit": power_limit(), "n_mesh": args.n_mesh,
+    gpu = timing.card()
+    result = {"card": gpu, "gpu": gpu["name"], "power_limit": gpu["power_limit"], "n_mesh": args.n_mesh,
               "rescaling": args.rescaling, "adaptation": args.adaptation, "bones": args.bones,
               "runs": []}
     e = torch.Tensor([])
@@ -94,56 +87,46 @@ def main():
             frame = lambda i: scenes.deform_base(mesh["verts"], 0.4 + 0.05 * (i % 12))
             pose_a = pose_b = lambda verts: verts
 
-        def route_a(x):
-            return fb.frosting_render_edited(params, edit, pose_a(x), rs, orig_quats=orig)
+        x = {}                                        # the frame every route of a step renders
 
-        def route_b(x):
+        def route_a():
+            return fb.frosting_render_edited(params, edit, pose_a(x["frame"]), rs, orig_quats=orig)
+
+        def route_b():
             a = scenes.edited_frosting_attributes(params, mesh["verts"], mesh["faces"], mesh["cells"], inner_dist,
-                                                  outer_dist, pose_b(x), rs.campos, 3, edition_mask=em,
+                                                  outer_dist, pose_b(x["frame"]), rs.campos, 3, edition_mask=em,
                                                   thickness_rescaling=args.rescaling, orig_quats=orig,
                                                   adaptation=args.adaptation, canonical=canonical)
             color, radii, _, _ = R._launch_forward(a["means3D"], e, a["colors_precomp"], a["opacities"], a["scales"],
                                                    a["rotations"], e, rs, None)
             return color, radii
 
-        def timed(routes, n):
-            times = {name: [] for name in routes}
-            outs = {}
-            with torch.no_grad():
-                for i in range(args.warmup):
-                    for name, fn in routes.items():
-                        outs[name] = fn(frame(i))
-                for i in range(n):
-                    x = frame(i)
-                    for name, fn in routes.items():
-                        torch.cuda.synchronize()
-                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                        e0.record()
-                        outs[name] = fn(x)
-                        e1.record()
-                        e1.synchronize()
-                        times[name].append(e0.elapsed_time(e1))
-            stats = {}
-            for name, t in times.items():
-                t = sorted(t)
-                stats[name] = {"median_ms": t[len(t) // 2], "min_ms": t[0], "max_ms": t[-1]}
-            return stats, outs
+        def timed(routes):
+            calls = itertools.count()
 
-        stats, outs = timed({"a_frosting_render_edited": route_a, "b_torch_chain_rasterizer": route_b}, args.iters)
+            def next_frame():       # made outside the timed window: frames 0, 1, ... over the warm-up, then from 0 again
+                i = next(calls) // len(routes)
+                x["frame"] = frame(i if i < args.warmup else i - args.warmup)
+
+            with torch.no_grad():
+                return timing.alternate(routes, args.iters, args.warmup, before=next_frame)
+
+        stats, outs = timed({"a_frosting_render_edited": route_a, "b_torch_chain_rasterizer": route_b})
         (ca, ra), (cb, rb) = outs["a_frosting_render_edited"], outs["b_torch_chain_rasterizer"]
         run = {"n_bg": n_bg, "rendered": int((ra > 0).sum()), "image_max_abs_diff": (ca - cb).abs().max().item(),
                "image_px_over_1e-4_frac": ((ca - cb).abs() > 1e-4).float().mean().item(),
                "radii_agree_frac": (ra == rb).float().mean().item(), **stats}
         run["speedup_b_over_a"] = run["b_torch_chain_rasterizer"]["median_ms"] / run["a_frosting_render_edited"]["median_ms"]
         if args.bones:
-            skin_stats, skin_outs = timed({"a_skin_cuda": pose_a, "b_skin_torch": pose_b}, args.iters)
+            skin_stats, skin_outs = timed({"a_skin_cuda": lambda: pose_a(x["frame"]),
+                                           "b_skin_torch": lambda: pose_b(x["frame"])})
             run["skin"] = dict(skin_stats, max_abs_diff=(skin_outs["a_skin_cuda"] - skin_outs["b_skin_torch"]).abs().max().item(),
                                speedup_b_over_a=skin_stats["b_skin_torch"]["median_ms"] / skin_stats["a_skin_cuda"]["median_ms"])
         result["runs"].append(run)
         print(json.dumps(run), flush=True)
         del params, mesh, outs, edit, canonical, pose_a, pose_b
         torch.cuda.empty_cache()
-    print(json.dumps(result))
+    timing.emit(result)
 
 
 if __name__ == "__main__":

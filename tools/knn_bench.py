@@ -10,13 +10,13 @@ Python call: allocation of the workspace and outputs, and the host read of the 4
 events enclose, so the times are upper bounds on the device work).  For context: scipy's cKDTree on the host up to 1 M
 distinct points (workers=-1, build + query, the route users have without pytorch3d; one timed call) and, at 200 k, an
 exhaustive chunked brute force in torch on the GPU (squared distances in matmul form + topk: every pair is scored, but
-not with the contract's float expression, so not bit-exact), a stand-in for pytorch3d's O(P^2) kernel.  Then, in a separate run under torch.profiler, the
-device time per kernel at 1 M.  The card's name and power limit are read in the same process.
+not with the contract's float expression, so not bit-exact), a stand-in for pytorch3d's O(P^2) kernel.  Then, in a
+separate run under the torch profiler, the device time per kernel at 1 M.  The card's name, power limit and max SM
+clock are read before and after the run.
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -24,40 +24,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from frosting_b200 import camera_batch, knn_points, scenes     # noqa: E402
+from tools import timing                                        # noqa: E402
 
 K = 16
-
-
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
-                            "0"], capture_output=True, text=True, timeout=20)
-        return r.stdout.strip() or "unknown"
-    except Exception:
-        return "unknown"
-
-
-def pct(t, q):
-    t = sorted(t)
-    return t[min(len(t) - 1, int(q * len(t)))]
-
-
-def summary(t):
-    return {"median_ms": round(pct(t, 0.5), 3), "p10_ms": round(pct(t, 0.1), 3), "p90_ms": round(pct(t, 0.9), 3)}
-
-
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    out = []
-    for _ in range(steps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        e1.synchronize()
-        out.append(e0.elapsed_time(e1))
-    return summary(out)
 
 
 def workload_points(name):
@@ -99,14 +68,14 @@ def main():
              ("C3 2M frosting centres", lambda: workload_points("c3")),
              ("C5 6M free Gaussians", lambda: workload_points("c5")),
              ("1M coincident", lambda: torch.full((1_000_000, 3), 0.5))]
-    res = {"card (name, power limit, max SM clock)": card(), "K": K, "cases": {}}
-    print(json.dumps({"card": res["card (name, power limit, max SM clock)"]}), flush=True)
+    gpu = timing.card()
+    res = {"card": gpu, "card (name, power limit, max SM clock)": ", ".join(gpu.values()), "K": K, "cases": {}}
     for name, make in cases:
         if a.cases is not None and not any(c in name for c in a.cases):
             continue
         pts = make()
         g = pts.to(dev)
-        row = {"P": len(pts), "knn_points": timed(lambda: knn_points(g, K=K), a.steps, a.warmup)}
+        row = {"P": len(pts), **timing.alternate({"knn_points": lambda: knn_points(g, K=K)}, a.steps, a.warmup)[0]}
         if len(pts) <= 1_000_000 and "coincident" not in name:     # cKDTree cannot split coincident points: O(P^2)
             from scipy.spatial import cKDTree
             t = time.perf_counter()
@@ -114,31 +83,16 @@ def main():
             row["cKDTree_host_ms"] = round(1e3 * (time.perf_counter() - t), 1)
             row["host_cpus"] = os.cpu_count()
         if len(pts) <= 200_000:
-            row["torch_brute_force"] = timed(lambda: brute_force(g), 3, 1)
+            row.update(timing.alternate({"torch_brute_force": lambda: brute_force(g)}, 3, 1)[0])
         res["cases"][name] = row
         print(json.dumps({name: row}), flush=True)
         del g
         torch.cuda.empty_cache()
     if not a.no_profile:
         g = scenes.knn_scene("sugar", 1_000_000, 1).to(dev)
-        for _ in range(3):
-            knn_points(g, K=K)
-        torch.cuda.synchronize()
-        from torch.profiler import ProfilerActivity, profile
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(a.steps):
-                knn_points(g, K=K)
-            torch.cuda.synchronize()
-        kern = {}
-        for ev in prof.key_averages():
-            if ev.device_type.name == "CUDA" and ev.count:
-                kern[ev.key[:90]] = {"calls": ev.count, "ms_per_call_total": round(ev.device_time_total / 1e3 / a.steps, 4)}
-        res["profile_sugar_1M_per_call"] = dict(sorted(kern.items(), key=lambda kv: -kv[1]["ms_per_call_total"]))
+        res["profile_sugar_1M_per_call"], _ = timing.kernel_times(lambda: knn_points(g, K=K), a.steps)
         print(json.dumps({"profile_sugar_1M_per_call": res["profile_sugar_1M_per_call"]}), flush=True)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            json.dump(res, f, indent=1)
+    timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

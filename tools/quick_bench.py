@@ -1,5 +1,6 @@
 """Developer timing script (not the contract bench): per-stage CUDA-event timings of frosting_b200 vs
-the compiled reference on random scenes.  Usage: python tools/quick_bench.py [P W H D]"""
+the compiled reference on random scenes, alternating, median of 10 after 3 warm-up rounds.
+Usage: python tools/quick_bench.py [P W H D]"""
 import sys
 import os
 import torch
@@ -8,19 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import frosting_b200 as fb
 from frosting_b200 import scenes
 from oracle import refdgr
-
-
-def timeit(fn, n=10, warm=3):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(n):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    ts.sort()
-    return ts[len(ts) // 2]
+from tools import timing
 
 
 def main():
@@ -57,10 +46,14 @@ def main():
     R = st["num_rendered"]
     print(f"P={P} {W}x{H} D={D} R={R} R/P={R / P:.2f} visible={(st['radii'] > 0).float().mean().item():.3f} "
           f"max_tile={int(st['tile_count'].max())}")
-    t_mf, t_mfb = timeit(mine_fwd), timeit(mine_fb)
+    routes = {"mine_fwd": mine_fwd, "mine_fb": mine_fb}
+    if refdgr.available():
+        routes.update(ref_fwd=ref_fwd, ref_fb=ref_fb)
+    t = {k: s["median_ms"] for k, s in timing.alternate(routes, 10, 3)[0].items()}
+    t_mf, t_mfb = t["mine_fwd"], t["mine_fb"]
     print(f"mine: fwd {t_mf:.3f} ms  fwd+bwd {t_mfb:.3f} ms  ({1000 / t_mfb:.1f} fps)")
     if refdgr.available():
-        t_rf, t_rfb = timeit(ref_fwd), timeit(ref_fb)
+        t_rf, t_rfb = t["ref_fwd"], t["ref_fb"]
         print(f"ref : fwd {t_rf:.3f} ms  fwd+bwd {t_rfb:.3f} ms  ({1000 / t_rfb:.1f} fps)")
         print(f"speedup fwd {t_rf / t_mf:.2f}x  fwd+bwd {t_rfb / t_mfb:.2f}x")
 

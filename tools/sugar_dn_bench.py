@@ -12,14 +12,13 @@ camera, a seeded ground-truth image.  Routes, alternating within each step, each
   (c) (a) plus the reference's structure: the features in torch, a second rasterizer call with them as colors_precomp
       and background 0, and the float32 torch loss (torch_reference_loss, the reference's lines).
 Reported: medians and p10/p90 over `--steps` steps after `--warmup`, (b) - (a) and (c) - (a) from the medians, the card
-and its power limit.  Then, in a separate run under torch.profiler (CUDA activity), the device time per step of each
+and its power limit.  Then, in a separate run under the torch profiler (CUDA activity), the device time per step of each
 kernel of (a) and of (b): the features kernels, the loss kernels, and the blend kernels of both, whose difference is the
 E = 3 extra-channel instance's cost over the colour-only one.
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -27,58 +26,12 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import frosting_b200 as fb                       # noqa: E402
 from frosting_b200 import scenes, sugar_dn       # noqa: E402
+from tools import timing                         # noqa: E402
 
 
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
-                            "0"], capture_output=True, text=True, timeout=20)
-        return r.stdout.strip() or "unknown"
-    except Exception:
-        return "unknown"
-
-
-def pct(t, q):
-    t = sorted(t)
-    return t[min(len(t) - 1, int(q * len(t)))]
-
-
-def summary(t):
-    return {"median_ms": round(pct(t, 0.5), 4), "p10_ms": round(pct(t, 0.1), 4), "p90_ms": round(pct(t, 0.9), 4)}
-
-
-def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1)
-
-
-GROUPS = (("features", ("dn_features_kernel", "dn_features_bwd_kernel")),
-          ("loss", ("dn_loss_fwd_kernel", "dn_loss_bwd_kernel")),
-          ("blend", ("render_fwd_pair_kernel", "render_bwd_t16_kernel", "extra_grad_kernel")))
-
-
-def kernel_times(fn, steps):
-    """Device time (ms) per step of each kernel / memset `fn` launches, from torch.profiler."""
-    from torch.profiler import ProfilerActivity, profile
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(steps):
-            fn()
-        torch.cuda.synchronize()
-    out = {}
-    for e in prof.key_averages():
-        t = getattr(e, "self_device_time_total", None)
-        if t is None:
-            t = e.self_cuda_time_total
-        if t > 0:
-            out[e.key[:100]] = round(out.get(e.key[:100], 0.0) + t / 1000.0 / steps, 4)
-    groups = {g: round(sum(v for k, v in out.items() if any(n in k for n in names)), 4) for g, names in GROUPS}
-    return out, groups
+GROUPS = {"features": ("dn_features_kernel", "dn_features_bwd_kernel"),
+          "loss": ("dn_loss_fwd_kernel", "dn_loss_bwd_kernel"),
+          "blend": ("render_fwd_pair_kernel", "render_bwd_t16_kernel", "extra_grad_kernel")}
 
 
 def workload(P, dev):
@@ -134,20 +87,14 @@ def workload(P, dev):
 def run(P, steps, warmup, dev):
     w = workload(P, dev)
     routes, losses = dict(zip("abc", w[:3])), w[3]
-    t = {k: [] for k in routes}
-    for i in range(warmup + steps):
-        for k, fn in routes.items():
-            ms = timed(fn)
-            if i >= warmup:
-                t[k].append(ms)
-    s = {k: summary(v) for k, v in t.items()}
+    s = timing.alternate(routes, steps, warmup)[0]
     out = {"P": P, "W": 1920, "H": 1080, "routes": s,
            "b_minus_a_ms": round(s["b"]["median_ms"] - s["a"]["median_ms"], 4),
            "c_minus_a_ms": round(s["c"]["median_ms"] - s["a"]["median_ms"], 4)}
     ours, f64 = losses()
     out["dn_loss"] = {"cuda": ours, "float64_reference": f64}
-    ka, ga = kernel_times(routes["a"], steps)
-    kb, gb = kernel_times(routes["b"], steps)
+    ka, ga = timing.kernel_times(routes["a"], steps, GROUPS)
+    kb, gb = timing.kernel_times(routes["b"], steps, GROUPS)
     out["profile_a"], out["profile_b"] = ka, kb
     out["groups_ms"] = {"features": gb["features"], "loss": gb["loss"], "blend_a": ga["blend"], "blend_b": gb["blend"],
                         "blend_extra": round(gb["blend"] - ga["blend"], 4)}
@@ -164,16 +111,12 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("sugar_dn_bench needs a CUDA device")
     dev = torch.device("cuda:0")
-    res = {"card": card(), "torch": torch.__version__, "runs": []}
+    res = {"card": timing.card(), "torch": torch.__version__, "runs": []}
     for P in a.sizes:
         r = run(P, a.steps, a.warmup, dev)
         print(json.dumps(r), flush=True)
         res["runs"].append(r)
-    res["card_after"] = card()
-    print(json.dumps({"card": res["card"], "card_after": res["card_after"]}))
-    if a.out:
-        with open(a.out, "w") as f:
-            json.dump(res, f, indent=1)
+    timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -10,8 +10,8 @@ the samples `sample_in_gaussians(mask, --samples)`.  Routes, alternating within 
   the sampler alone; one rasterizer frame (forward + backward) on the same scene, for scale;
   and the op's own pieces: forward without gradient, forward with gradient (the per-pair pass also differentiating),
   backward (the per-Gaussian chain kernel).
-These are call times: CUDA events around the Python call, host work included.  Then, in a separate run under
-torch.profiler (CUDA activity), the device time of each of the op's kernels over `--steps` steps of forward with
+These are call times: CUDA events around the Python call, host work included.  Then, in a separate run under the
+torch profiler (CUDA activity), the device time of each of the op's kernels over `--steps` steps of forward with
 gradient + backward and of forward without gradient (inputs detached, so the gradient pass is not asked for).
 Medians and p10/p90 over `--steps` timed steps after `--warmup`; each route's peak extra memory; the agreement of (a)
 with (b); the card and its power limit; the sample kernel's bytes over its own device time.
@@ -19,7 +19,6 @@ with (b); the card and its power limit; the sample kernel's bytes over its own d
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -27,35 +26,9 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import frosting_b200 as fb                       # noqa: E402
 from frosting_b200 import scenes, sugar          # noqa: E402
+from tools import timing                         # noqa: E402
 
 LEAVES = ("points", "scaling", "quaternions", "strengths")
-
-
-def card():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
-                            "0"], capture_output=True, text=True, timeout=20)
-        return r.stdout.strip() or "unknown"
-    except Exception:
-        return "unknown"
-
-
-def pct(t, q):
-    t = sorted(t)
-    return t[min(len(t) - 1, int(q * len(t)))]
-
-
-def summary(t):
-    return {"median_ms": round(pct(t, 0.5), 4), "p10_ms": round(pct(t, 0.1), 4), "p90_ms": round(pct(t, 0.9), 4)}
-
-
-def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    out = fn()
-    e1.record()
-    e1.synchronize()
-    return out, e0.elapsed_time(e1)
 
 
 def peak(fn):
@@ -79,23 +52,11 @@ def kernel_name(key):
     return "memset" if "Memset" in key else key[:80]
 
 
-def kernel_times(fn, steps):
-    """Mean device time (ms) per step of each kernel / memset that `fn` launches, from torch.profiler."""
-    from torch.profiler import ProfilerActivity, profile
-    fn()
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(steps):
-            fn()
-        torch.cuda.synchronize()
+def by_kernel(kernels):
+    """`timing.kernel_times`' table with the op's kernels and the memsets each summed under one name."""
     out = {}
-    for e in prof.key_averages():
-        t = getattr(e, "self_device_time_total", None)
-        if t is None:
-            t = e.self_cuda_time_total
-        if t > 0:
-            name = kernel_name(e.key)
-            out[name] = round(out.get(name, 0.0) + t / 1000.0 / steps, 4)
+    for key, ms in kernels.items():
+        out[kernel_name(key)] = round(out.get(kernel_name(key), 0.0) + ms, 4)
     return out
 
 
@@ -141,27 +102,19 @@ def run(P, N, steps, warmup, dev):
         with torch.no_grad():
             return sugar.sdf_regularization(*leaves, nb, idx, eps)
 
+    held = {}
+
     def fwd_grad():
-        return sugar.sdf_regularization(*leaves, nb, idx, eps)
+        held["terms"] = sugar.sdf_regularization(*leaves, nb, idx, eps)
+        return held["terms"]
+
+    def bwd():                           # the backward alone, over the forward the route before it made
+        est, nrm = held.pop("terms")
+        return torch.autograd.grad(0.2 * est + 0.2 * nrm, leaves)
 
     routes = {"cuda_fwd_bwd": ours, "torch_fwd_bwd": ref, "sampler": lambda: sugar.sample_in_gaussians(mask, N),
-              "raster_frame": frame, "cuda_fwd_nograd": fwd_nograd, "cuda_fwd_grad": fwd_grad}
-    times = {k: [] for k in (*routes, "cuda_bwd")}
-    held = None
-    for step in range(warmup + steps):
-        for name, fn in routes.items():
-            torch.cuda.synchronize()
-            _, ms = timed(fn)
-            if step >= warmup:
-                times[name].append(ms)
-        # the backward alone, over a forward made outside the timed window
-        est, nrm = fwd_grad()
-        torch.cuda.synchronize()
-        _, ms = timed(lambda: torch.autograd.grad(0.2 * est + 0.2 * nrm, leaves))
-        if step >= warmup:
-            times["cuda_bwd"].append(ms)
-        held = (est, nrm)
-    del held
+              "raster_frame": frame, "cuda_fwd_nograd": fwd_nograd, "cuda_fwd_grad": fwd_grad, "cuda_bwd": bwd}
+    call_times = timing.alternate(routes, steps, warmup)[0]
     (to, go), mem_ours = peak(ours)
     (tr, gr), mem_ref = peak(ref)
     agree = {"terms_rel": [abs(float(a.detach() - b.detach())) / max(abs(float(b.detach())), 1e-30) for a, b in zip(to, tr)],
@@ -173,8 +126,8 @@ def run(P, N, steps, warmup, dev):
         est, nrm = sugar.sdf_regularization(*leaves, nb, idx, eps)
         torch.autograd.grad(0.2 * est + 0.2 * nrm, leaves)
 
-    kt_grad = kernel_times(step_grad, steps)
-    kt_nograd = kernel_times(lambda: sugar.sdf_regularization(*detached, nb, idx, eps), steps)
+    kt_grad = by_kernel(timing.kernel_times(step_grad, steps)[0])
+    kt_nograd = by_kernel(timing.kernel_times(lambda: sugar.sdf_regularization(*detached, nb, idx, eps), steps)[0])
     M, K = int(mask.sum()), nb.K
     # bytes of the per-pair pass (the with-gradient forward): per pair one 80-byte record gather and five 16-byte
     # vector reductions; per sample the draws (20 B), the owner's quaternion, scales, record and table row, and five
@@ -183,7 +136,7 @@ def run(P, N, steps, warmup, dev):
     dram_min = P * (12 + 12 + 16 + 4 + 4 * K + 80 + 128 + 44) + N * 20
     ms_pairs = kt_grad["sugar_sample_kernel<grad>"]
     return {"P": P, "K": K, "N": N, "masked": M,
-            "call_times": {k: summary(v) for k, v in times.items()},
+            "call_times": call_times,
             "kernels_fwd_grad_plus_bwd_ms": kt_grad, "kernels_fwd_nograd_ms": kt_nograd,
             "peak_extra_bytes": {"cuda": mem_ours, "torch": mem_ref},
             "agreement": agree,
@@ -203,15 +156,12 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("sugar_reg_bench needs a CUDA device")
     dev = torch.device("cuda:0")
-    res = {"card": card(), "torch": torch.__version__, "runs": []}
+    res = {"card": timing.card(), "torch": torch.__version__, "runs": []}
     for P in a.sizes:
         r = run(P, a.samples, a.steps, a.warmup, dev)
         print(json.dumps(r), flush=True)
         res["runs"].append(r)
-    print(json.dumps({"card": res["card"]}))
-    if a.out:
-        with open(a.out, "w") as f:
-            json.dump(res, f, indent=1)
+    timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

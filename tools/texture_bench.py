@@ -14,10 +14,8 @@ colours).  With `--obj-dir`, `write_textured_obj` of route (a)'s result is timed
 Reports the medians, the agreement of the two routes' textures, and the card and its power limit.
 """
 import argparse
-import json
 import math
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -29,30 +27,7 @@ import frosting_b200 as fb                       # noqa: E402
 from frosting_b200 import scenes                 # noqa: E402
 from frosting_b200.mesh import MeshRasterizer, rasterize_mesh   # noqa: E402
 from frosting_b200.texture import _settings, render_view      # noqa: E402
-
-
-def power_limit():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=20)
-        return r.stdout.strip() or "unknown"
-    except Exception:
-        return "unknown"
-
-
-def stats(t):
-    t = sorted(t)
-    return {"median_ms": t[len(t) // 2], "min_ms": t[0], "max_ms": t[-1]}
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    out = fn()
-    e1.record()
-    e1.synchronize()
-    return out, e0.elapsed_time(e1)
+from tools import timing                                       # noqa: E402
 
 
 def main():
@@ -74,7 +49,8 @@ def main():
     verts, faces = mesh["verts"], mesh["faces"]
     bg = torch.zeros(3, device=dev)
     F = faces.shape[0]
-    result = {"gpu": torch.cuda.get_device_name(dev), "power_limit": power_limit(), "n_mesh": args.n_mesh,
+    gpu = timing.card()
+    result = {"card": gpu, "gpu": gpu["name"], "power_limit": gpu["power_limit"], "n_mesh": args.n_mesh,
               "n_faces": F, "cameras": args.cameras, "image": [W, H], "square_size": sq,
               "texture_size": sq * int(math.sqrt(F // 2 + 1) + 1)}
 
@@ -92,17 +68,10 @@ def main():
             barys.append(frag.bary_coords.view(H, W, 3))
         return scenes.bake_texture_torch(F, mesh["cells"], params["sh_dc"], sq, images, p2fs, barys)[2]
 
-    times = {"a_compute_textured_mesh": [], "b_torch_bake": []}
-    outs = {}
     with torch.no_grad():
-        for i in range(args.warmup + args.iters):
-            for name, fn in (("a_compute_textured_mesh", route_a), ("b_torch_bake", route_b)):
-                outs.pop(name, None)
-                outs[name], ms = timed(fn)
-                if i >= args.warmup:
-                    times[name].append(ms)
-        for name, t in times.items():
-            result[name] = stats(t)
+        times, outs = timing.alternate({"a_compute_textured_mesh": route_a, "b_torch_bake": route_b}, args.iters,
+                                       args.warmup)
+        result.update(times)
         result["speedup_b_over_a"] = result["b_torch_bake"]["median_ms"] / result["a_compute_textured_mesh"]["median_ms"]
         ta, tb = outs["a_compute_textured_mesh"], outs["b_torch_bake"]
         result["texels_equal_frac"] = (ta == tb).all(dim=-1).float().mean().item()
@@ -117,23 +86,23 @@ def main():
             img = render_view(params, mesh, _settings(cam, 0, bg, dev))
             views.append((cam, p2f, img.permute(1, 2, 0).contiguous()))
         stage = {"setup": [], "mesh_bary": [], "add_view": [], "finish": []}
+
+        def timed(name, fn):
+            ms, out = timing.timed(fn)
+            stage[name].append(ms)
+            return out
+
         for i in range(args.warmup + args.iters):
-            baker, ms = timed(lambda: fb.TextureBaker(faces, mesh["cells"], params["sh_dc"], verts.shape[0], sq))
-            keep = i >= args.warmup
-            if keep:
-                stage["setup"].append(ms)
+            if i == args.warmup:                  # the warm-up passes' times are dropped
+                for t in stage.values():
+                    t.clear()
+            baker = timed("setup", lambda: fb.TextureBaker(faces, mesh["cells"], params["sh_dc"], verts.shape[0], sq))
             for cam, p2f, img in views:
-                bary, ms = timed(lambda: fb.mesh_bary(verts, faces, cam.full_proj_transform, p2f))
-                if keep:
-                    stage["mesh_bary"].append(ms)
-                _, ms = timed(lambda: baker.add_view(img, p2f, bary))
-                if keep:
-                    stage["add_view"].append(ms)
-            (_, _, tex), ms = timed(baker.finish)
-            if keep:
-                stage["finish"].append(ms)
-            del baker, tex
-        result["stages"] = {k: stats(v) for k, v in stage.items()}
+                bary = timed("mesh_bary", lambda: fb.mesh_bary(verts, faces, cam.full_proj_transform, p2f))
+                timed("add_view", lambda: baker.add_view(img, p2f, bary))
+            timed("finish", baker.finish)
+            del baker
+        result["stages"] = {k: timing.summary(v) for k, v in stage.items()}
         result["hit_pixels_per_view"] = sum(int((p2f >= 0).sum()) for _, p2f, _ in views) / len(views)
         del views
 
@@ -146,7 +115,7 @@ def main():
                 paths = fb.write_textured_obj(os.path.join(d, "frosting_textured.obj"), **out)
                 result["write_obj_s"] = time.perf_counter() - t0
                 result["obj_bytes"] = {os.path.basename(p): os.path.getsize(p) for p in paths}
-    print(json.dumps(result))
+    timing.emit(result)
 
 
 if __name__ == "__main__":
