@@ -111,6 +111,17 @@ class SugarReg(C.Structure):
                                           "d_eps", "d_workspace")]
 
 
+class FrostingInit(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_verts", "n_faces", "P", "K", "n_samples", "smooth_K", "std_K")] + \
+               [(n, C.c_float) for n in ("level", "std_range", "min_layer", "half_layer")] + \
+               [(n, C.c_void_p) for n in ("d_verts", "d_faces", "d_vf_offsets", "d_vf_faces", "d_normals", "d_points",
+                                          "d_scaling", "d_quaternions", "d_strengths", "d_knn_idx", "d_std_idx",
+                                          "d_inner_range", "d_outer_range", "d_min_clamp_inner", "d_max_clamp_outer",
+                                          "d_fractions", "d_smooth_idx", "d_level_outer", "d_level_inner",
+                                          "d_outer_dist", "d_inner_dist", "d_outer_verts", "d_inner_verts",
+                                          "d_densities")]
+
+
 ADAM_MAX_GROUPS = 16
 MAX_PEERS = 8
 PEER_HANDLE_BYTES = 64
@@ -172,6 +183,7 @@ ABI_STRUCTS = (
     ("fb200_extra", Extra), ("fb200_frosting_params", FrostingParams), ("fb200_frosting_grads", FrostingGrads),
     ("fb200_adam_args", AdamArgs), ("fb200_layout", Layout), ("fb200_frosting_edit", FrostingEdit),
     ("fb200_frosting_skin", FrostingSkin), ("fb200_texture", Texture), ("fb200_sugar_reg", SugarReg),
+    ("fb200_frosting_init", FrostingInit),
 )
 
 _i32, _i64, _f32, _vp, _int, _size = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_int, C.c_size_t
@@ -216,6 +228,7 @@ SIGNATURES = {
     "fb200_sugar_dn_loss_backward": (_int, [_vp, _i32, _i32] + [_vp] * 5),
     "fb200_knn_workspace_bytes": (_size, [_i32, _i32, _i32]),
     "fb200_knn": (_int, [_vp, _i32, _vp, _i32, _i32, _vp, _size, _vp, _vp, _vp]),
+    "fb200_level_points": (_int, [C.POINTER(FrostingInit), _vp]),
     "fb200_adam_step": (_int, [C.POINTER(AdamArgs), _vp]),
     "fb200_peer_alloc": (_int, [_size, C.POINTER(_vp)]),
     "fb200_peer_free": (_int, [_vp]),

@@ -15,7 +15,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libfrosting_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "geom_bwd.cu", "mesh_vis.cu",
            "frosting_attr.cu", "frosting_edit.cu", "frosting_skin.cu", "texture.cu", "loss.cu", "optim.cu", "sugar_reg.cu",
-           "sugar_dn.cu", "knn.cu"]
+           "sugar_dn.cu", "knn.cu", "frosting_init.cu"]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [

@@ -297,7 +297,8 @@ int fb200_abi_struct_sizes(size_t* out) {
                                              sizeof(fb200_grads), sizeof(fb200_extra), sizeof(fb200_frosting_params),
                                              sizeof(fb200_frosting_grads), sizeof(fb200_adam_args), sizeof(fb200_layout),
                                              sizeof(fb200_frosting_edit), sizeof(fb200_frosting_skin),
-                                             sizeof(fb200_texture), sizeof(fb200_sugar_reg)};
+                                             sizeof(fb200_texture), sizeof(fb200_sugar_reg),
+                                             sizeof(fb200_frosting_init)};
     for (int i = 0; i < FB200_ABI_STRUCTS; ++i) out[i] = sizes[i];
     return FB200_OK;
 }
@@ -798,6 +799,36 @@ int fb200_knn(const float* d_points, int32_t P, const float* d_queries, int32_t 
     }
     return check(launch_knn(d_points, P, d_queries, Q, K, d_workspace, d_dists, d_idx, static_cast<cudaStream_t>(stream)),
                  "knn");
+}
+
+// fb200_level_points: extents and the pointers each requested stage reads or writes
+static int check_level_points(const fb200_frosting_init* lp) {
+    if (!lp) return fail(FB200_EINVAL, "level_points: null struct");
+    if (lp->n_verts < 0 || lp->P < 1 || lp->K < 1 || lp->K > 32 || lp->K > lp->P || lp->n_samples < 1 ||
+        lp->n_samples > 32 || lp->smooth_K < 0 || lp->smooth_K > 32 || lp->std_K < 0 || lp->std_K > 32)
+        return fail(FB200_EINVAL, "level_points: bad extents (V >= 0, 1 <= K <= min(32, P), 1 <= n_samples <= 32, "
+                                  "0 <= smooth_K, std_K <= 32)");
+    if (lp->n_verts == 0) return FB200_OK;
+    if (!lp->d_verts || !lp->d_normals || !lp->d_points || !lp->d_scaling || !lp->d_quaternions || !lp->d_strengths ||
+        !lp->d_knn_idx || !lp->d_inner_range || !lp->d_outer_range || !lp->d_fractions)
+        return fail(FB200_EINVAL, "level_points: missing input pointer");
+    if (lp->d_faces && (lp->n_faces < 1 || !lp->d_vf_offsets || !lp->d_vf_faces))
+        return fail(FB200_EINVAL, "level_points: the normals stage needs n_faces >= 1 and the vertex -> face table");
+    if (lp->d_std_idx && lp->std_K < 1) return fail(FB200_EINVAL, "level_points: the proposal stage needs std_K >= 1");
+    if ((lp->smooth_K > 0) != (lp->d_smooth_idx != nullptr))
+        return fail(FB200_EINVAL, "level_points: give the smoothing table exactly when smooth_K > 0");
+    if (!(lp->min_layer >= 0.f) || !(lp->half_layer >= 0.f))
+        return fail(FB200_EINVAL, "level_points: min_layer and half_layer must be >= 0");
+    if (!lp->d_level_outer || !lp->d_level_inner || !lp->d_outer_dist || !lp->d_inner_dist || !lp->d_outer_verts ||
+        !lp->d_inner_verts)
+        return fail(FB200_EINVAL, "level_points: missing output pointer");
+    return FB200_OK;
+}
+
+int fb200_level_points(const fb200_frosting_init* lp, void* stream) {
+    int rc = check_level_points(lp);
+    if (rc != FB200_OK) return rc;
+    return check(launch_level_points(*lp, static_cast<cudaStream_t>(stream)), "level_points");
 }
 
 int fb200_adam_step(const fb200_adam_args* a, void* stream) {

@@ -31,6 +31,7 @@
 #include "common.cuh"
 #include "frosting_attr.cuh"
 #include "sh.cuh"
+#include "vec3.cuh"
 
 namespace fb200 {
 
@@ -42,20 +43,6 @@ constexpr int kSelBelow = kSelectBins;                // d_select words after th
 constexpr int kSelPrefix = kSelectBins + 1;
 constexpr int kSelMask = kSelectBins + 2;
 
-struct V3 { float x, y, z; };
-
-__device__ __forceinline__ V3 ld3(const float* p) { return {__ldg(p), __ldg(p + 1), __ldg(p + 2)}; }
-__device__ __forceinline__ V3 sub(V3 a, V3 b) { return {fadd(a.x, -b.x), fadd(a.y, -b.y), fadd(a.z, -b.z)}; }
-__device__ __forceinline__ V3 cross(V3 a, V3 b) {
-    return {fadd(fmul(a.y, b.z), -fmul(a.z, b.y)), fadd(fmul(a.z, b.x), -fmul(a.x, b.z)),
-            fadd(fmul(a.x, b.y), -fmul(a.y, b.x))};
-}
-__device__ __forceinline__ float norm3(V3 a) { return __fsqrt_rn(fadd(fadd(fmul(a.x, a.x), fmul(a.y, a.y)), fmul(a.z, a.z))); }
-// x / max(|x|, eps): F.normalize and pytorch3d's normal normalisations
-__device__ __forceinline__ V3 normalize_eps(V3 a, float eps) {
-    const float n = fmaxf(norm3(a), eps);
-    return {__fdiv_rn(a.x, n), __fdiv_rn(a.y, n), __fdiv_rn(a.z, n)};
-}
 __device__ __forceinline__ float median3(float a, float b, float c) { return fmaxf(fminf(a, b), fminf(fmaxf(a, b), c)); }
 
 // quaternions (w, x, y, z) as float4 (x = w)
@@ -119,8 +106,7 @@ edit_face_kernel(fb200_frosting_edit e) {
     V3 v[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) { vid[k] = __ldg(e.d_faces + 3 * f + k); v[k] = ld3(e.d_base_verts + 3 * (size_t)vid[k]); }
-    // vertex-normal contribution (Meshes._compute_vertex_normals): cross(v2 - v1, v0 - v1), |.| = twice the area
-    const V3 an = cross(sub(v[2], v[1]), sub(v[0], v[1]));
+    const V3 an = area_normal(v[0], v[1], v[2]);
     e.d_face_normals[3 * f] = an.x; e.d_face_normals[3 * f + 1] = an.y; e.d_face_normals[3 * f + 2] = an.z;
     // face frame [n, normalize(v0 - v1), normalize(n x R1)] -> quaternion (compute_face_quaternions)
     const V3 r0 = normalize_eps(normalize_eps(cross(sub(v[1], v[0]), sub(v[2], v[0])), 1e-6f), 1e-12f);

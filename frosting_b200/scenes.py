@@ -844,3 +844,36 @@ def knn_scene(kind, P, seed, outlier_frac=0.01):
         d = torch.nn.functional.normalize(torch.randn(P, 3, generator=g), dim=-1)
         return (torch.tensor([1000.0, 1000.0, 1000.0]) + r * d).contiguous()
     raise ValueError(f"unknown knn scene {kind!r}; one of {KNN_SCENES}")
+
+
+# ---- Frosting initialisation scenes (frosting_init.py): a base mesh inside a SuGaR surface and a 3DGS cloud ----
+
+def frosting_init_scene(n_verts, n_sugar, n_gs, seed, radius=2.0, centre=(0.0, 0.0, 6.0)):
+    """A UV-sphere base mesh of about n_verts vertices (radius `radius` around `centre`) with the two Gaussian sets
+    Frosting.__init__ reads, activated, on the CPU: `sugar`, n_sugar flat SuGaR Gaussians on the sphere (thin axis
+    along the normal, 0.3 % radial jitter) and `gs`, n_gs 3DGS Gaussians in a shell of 4 % radial jitter around it, random
+    orientations.  Each is (points [P,3], scaling [P,3], unit quaternions [P,4], strengths [P,1])."""
+    n_lat = max(3, int(round(math.sqrt(n_verts / 2))))
+    n_lon = max(3, int(round((n_verts - 2) / (n_lat - 1))))
+    verts, faces, _ = uv_sphere(n_lat, n_lon, radius=radius, centre=centre)
+    g = torch.Generator().manual_seed(seed)
+    c = torch.tensor(centre)
+
+    def on_sphere(P, jitter):
+        d = torch.nn.functional.normalize(torch.randn(P, 3, generator=g), dim=-1)
+        return d, c + (radius + jitter * torch.randn(P, 1, generator=g)) * d
+
+    spacing = math.sqrt(4 * math.pi * radius ** 2 / max(n_sugar, 1))
+    d, pts = on_sphere(n_sugar, 0.003 * radius)
+    t1 = torch.nn.functional.normalize(torch.linalg.cross(d, torch.randn(n_sugar, 3, generator=g), dim=-1), dim=-1)
+    R = torch.stack([d, t1, torch.linalg.cross(d, t1, dim=-1)], -1)           # column 0: the normal
+    scaling = spacing * torch.exp(0.3 * torch.randn(n_sugar, 3, generator=g))
+    scaling[:, 0] = spacing * 0.05 * torch.exp(0.3 * torch.randn(n_sugar, generator=g))
+    sugar = (pts, scaling, matrix_to_quaternion(R), torch.sigmoid(1.5 + torch.randn(n_sugar, 1, generator=g)))
+    spacing_gs = math.sqrt(4 * math.pi * radius ** 2 / max(n_gs, 1))
+    _, pts = on_sphere(n_gs, 0.04 * radius)
+    gs = (pts, 0.5 * spacing_gs * torch.exp(0.4 * torch.randn(n_gs, 3, generator=g)),
+          torch.nn.functional.normalize(torch.randn(n_gs, 4, generator=g), dim=-1),
+          torch.sigmoid(torch.randn(n_gs, 1, generator=g)))
+    return dict(verts=verts, faces=faces, sugar=tuple(t.float().contiguous() for t in sugar),
+                gs=tuple(t.float().contiguous() for t in gs), spatial_extent=2.0 * radius)

@@ -514,6 +514,64 @@ size_t fb200_knn_workspace_bytes(int32_t P, int32_t Q, int32_t K);
 int fb200_knn(const float* d_points, int32_t P, const float* d_queries, int32_t Q, int32_t K, void* d_workspace,
               size_t workspace_bytes, float* d_dists, int64_t* d_idx, void* stream);
 
+/* Frosting layer thickness: the level crossings of a Gaussian density field along the base mesh's vertex normals
+ * (frosting_model.py compute_level_points_along_normals, :2016-2208, use_last_intersection_as_inner_level_point=True;
+ * called twice by Frosting.__init__, :296-369).  One call runs, in order:
+ *   normals   (d_faces given) d_normals[v] = the area-weighted normals cross(v2 - v1, v0 - v1) of the faces listed for v
+ *             in the CSR d_vf_offsets / d_vf_faces, summed in that order and normalised with eps 1e-6 (pytorch3d's
+ *             Meshes.verts_normals); otherwise d_normals is an input;
+ *   proposal  (d_std_idx given) s_v = mean over the std_K Gaussians g = d_std_idx[v,k] of
+ *             |scaling_g * quaternion_apply(quaternion_invert(q_g), n_v)| (pytorch3d's raw products), then
+ *             d_inner_range[v] = std_range s_v and d_outer_range[v] = -std_range s_v; otherwise both are inputs;
+ *   levels    t_j = f_j (inner_range - outer_range) + outer_range with f = d_fractions [n_samples] (torch.linspace(0, 1,
+ *             n) as computed by the caller), sample x_j = vert + t_j n; over the K Gaussians g = d_knn_idx[v,k] in table
+ *             order, d_j = sum_k strength_g exp(-clamp(|A_g^T (x_j - mu_g)|^2, 0, 1e8) / 2) with A_g =
+ *             quaternion_to_matrix(q_g) diag(1 / clamp(s_g, 1e-8)), and d_j >= 1 becomes d_j / (d_j + 1e-12).  outer:
+ *             linear interpolation of the level before the first sample above it, t_0 when that is sample 0; inner: after
+ *             the last sample above it, t_{n-1} when that is sample n-1; a vertex with no sample above the level and
+ *             d_0 < level gets (inner_range + outer_range) / 2 for both; then a layer thinner than min_layer is replaced
+ *             by (inner_range + outer_range) / 2 -/+ half_layer, then inner = max(inner, d_min_clamp_inner) and outer =
+ *             min(outer, d_max_clamp_outer) where given.  Written to d_level_outer / d_level_inner, d_densities [V,n] d_j
+ *             where given;
+ *   smoothing d_outer_dist[v] = the mean of d_level_outer over the smooth_K vertices d_smooth_idx[v,:] (smooth_K = 0:
+ *             the value itself), likewise inner; d_outer_verts / d_inner_verts [V,3] = vert + dist n.
+ * Extents: V >= 0, P >= 1, 1 <= K <= 32, K <= P, 1 <= n_samples <= 32, 0 <= smooth_K <= 32, 0 <= std_K <= 32 (>= 1 with
+ * d_std_idx).  The neighbour tables are not checked and must lie in [0, P) (Gaussians) or [0, V) (vertices).  Every
+ * array is float32 row-major unless marked; quaternions (w, x, y, z) raw, strengths [P] or [P,1].  Stream-ordered, no
+ * host synchronisation, no allocation, no atomics: the outputs depend on the input bits alone. */
+typedef struct fb200_frosting_init {
+    int32_t n_verts, n_faces, P, K, n_samples, smooth_K, std_K;
+    float level;
+    float std_range;
+    float min_layer;                    /* min_layer_size * spatial_extent rounded to float32, 0: none */
+    float half_layer;                   /* 0.5 * min_layer_size * spatial_extent rounded to float32 */
+    const float* d_verts;               /* [V,3] */
+    const int32_t* d_faces;             /* [F,3] or NULL: d_normals is an input */
+    const int32_t* d_vf_offsets;        /* [V+1] with d_faces */
+    const int32_t* d_vf_faces;          /* [3F] with d_faces */
+    float* d_normals;                   /* [V,3] */
+    const float* d_points;              /* [P,3] */
+    const float* d_scaling;             /* [P,3] activated */
+    const float* d_quaternions;         /* [P,4] */
+    const float* d_strengths;           /* [P] activated */
+    const int64_t* d_knn_idx;           /* [V,K] */
+    const int64_t* d_std_idx;           /* [V,std_K] or NULL: the ranges are inputs */
+    float* d_inner_range;               /* [V] */
+    float* d_outer_range;               /* [V] */
+    const float* d_min_clamp_inner;     /* [V] or NULL */
+    const float* d_max_clamp_outer;     /* [V] or NULL */
+    const float* d_fractions;           /* [n_samples] */
+    const int64_t* d_smooth_idx;        /* [V,smooth_K], NULL when smooth_K = 0 */
+    float* d_level_outer;               /* [V] */
+    float* d_level_inner;               /* [V] */
+    float* d_outer_dist;                /* [V] */
+    float* d_inner_dist;                /* [V] */
+    float* d_outer_verts;               /* [V,3] */
+    float* d_inner_verts;               /* [V,3] */
+    float* d_densities;                 /* [V,n_samples] or NULL */
+} fb200_frosting_init;
+int fb200_level_points(const fb200_frosting_init* lp, void* stream);
+
 /* Data-parallel gradient reduction fused with the Adam update (SURVEY.md row f3).  Replaces "all-reduce every
  * .grad, then torch.optim.Adam(l, lr=0.0, eps=1e-15).step()" (frosting_scene/frosting_optimizer.py:101,116-118) for
  * camera-sharded training.  All learnable tensors of a rank live in ONE flat fp32 parameter slab and their gradients
@@ -618,9 +676,10 @@ int64_t fb200_kernel_launches(void);
 const char* fb200_last_error(void);
 int fb200_abi_version(void);
 /* sizeof() of the ABI structs, in this order: {params, inputs, workspace, grads, extra, frosting_params,
- * frosting_grads, adam_args, layout, frosting_edit, frosting_skin, texture, sugar_reg}: lets a foreign-language binding
- * verify its struct mirrors at load time.  Check fb200_abi_version() first: the count grows with the version. */
-#define FB200_ABI_STRUCTS 13
+ * frosting_grads, adam_args, layout, frosting_edit, frosting_skin, texture, sugar_reg, frosting_init}: lets a
+ * foreign-language binding verify its struct mirrors at load time.  `out` holds FB200_ABI_STRUCTS entries of this
+ * header; structs are only ever appended to the list. */
+#define FB200_ABI_STRUCTS 14
 int fb200_abi_struct_sizes(size_t* out /* [FB200_ABI_STRUCTS] */);
 
 #ifdef __cplusplus
