@@ -22,6 +22,7 @@ CASES = {
     "min_layer": [(0.0, 0.02, 0.02), TINY],
     "clamp_inner": [(0.0, 0.2, 0.5), TINY],
     "clamp_outer": [(0.0, 0.2, 0.5), TINY],
+    "ends": [(-1.0, 0.02, 0.5), (1.0, 0.02, 0.5)],        # above only at samples 0 and n - 1: both crossings bound
 }
 
 
@@ -85,6 +86,8 @@ def test_edge_branches_in_the_float64_model():
     assert out["first"][at["one_crossing"]] > 0 and out["last"][at["one_crossing"]] == N_SAMPLES - 1
     assert out["d"][at["saturated"]].max() == pytest.approx(1.0, abs=1e-9)
     assert out["flat"][at["min_layer"]] and out["flat"].sum() == 1 + 2     # the two empty vertices have width 0 too
+    assert (out["first"][at["ends"]], out["last"][at["ends"]]) == (0, N_SAMPLES - 1) and not out["empty"][at["ends"]]
+    assert (out["d"][at["ends"]] > LEVEL).sum() == 2
     check_edge_values(sc["names"], out["outer_raw"], out["inner_raw"], 1e-12)
     # every sample is decided: more than 1e-5 from the level
     assert (np.abs(out["d"] - LEVEL) > 1e-5).all()
@@ -167,3 +170,142 @@ def test_c_boundary_rejects_bad_extents_without_touching_cuda():
     assert L.fb200_level_points(None, None) == -1
     st = _lib.FrostingInit(**dict(base, n_verts=0))
     assert L.fb200_level_points(C.byref(st), None) == 0          # nothing to do: no launch
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The staged model (normals, proposal, level stage with magnitudes) against the torch restatement in float64
+
+FAN = 70                  # valence of the fan's centre vertex
+ISOLATED, ZERO_AREA = FAN + 1, (FAN + 2, FAN + 3, FAN + 4)
+
+
+def hand_mesh():
+    """75 vertices (8 k + 3): a fan of FAN triangles around vertex 0 (its first five faces duplicated), an isolated
+    vertex, and three vertices whose only faces have zero area (two of them coincide).  The Gaussians (SuGaR and 3DGS
+    alike) have non-unit quaternions and some scales under the 1e-8 clamp; at the isolated vertex sits one of strength
+    exactly the float32 level with scales (0, 1e-9, 1e-8) -- every sample of a zero-normal vertex is the vertex itself --
+    and its other nearest Gaussians, a distance 1 away with scales <= 1e-7, underflow through the 1e8 clamp.
+    Returns float32 CPU tensors."""
+    g = torch.Generator().manual_seed(5)
+    th = 2 * np.pi * torch.arange(FAN, dtype=torch.float64) / FAN
+    ring = torch.stack([th.cos(), th.sin(), 0.05 * (3 * th).sin()], -1)
+    verts = torch.cat([torch.zeros(1, 3, dtype=torch.float64), ring,
+                       torch.tensor([[10.0, 0, 0], [20.0, 0, 0], [20.0, 1.0, 0], [20.0, 0, 0]], dtype=torch.float64)])
+    fan = torch.stack([torch.zeros(FAN, dtype=torch.long), 1 + torch.arange(FAN), 1 + (torch.arange(FAN) + 1) % FAN], -1)
+    z = ZERO_AREA
+    faces = torch.cat([fan, fan[:5], torch.tensor([[z[0], z[0], z[1]], [z[1], z[2], z[0]]])]).to(torch.int32)
+    n_fan = 48
+    r, a = 1.1 * torch.rand(n_fan, generator=g).sqrt(), 2 * np.pi * torch.rand(n_fan, generator=g)
+    pts = torch.cat([torch.stack([r * a.cos(), r * a.sin(), 0.03 * torch.randn(n_fan, generator=g)], -1),
+                     torch.tensor([[10.0, 0, 0], [10.0, 1.0, 0], [10.0, -1.0, 0], [10.0, 0, 1.0], [20.0, 0.5, 0],
+                                   [20.5, 1.0, 0]])])
+    scl = torch.cat([torch.stack([0.3 * torch.exp(0.3 * torch.randn(n_fan, generator=g)),
+                                  0.3 * torch.exp(0.3 * torch.randn(n_fan, generator=g)),
+                                  0.02 * torch.exp(0.3 * torch.randn(n_fan, generator=g))], -1),
+                     torch.tensor([[0.0, 1e-9, 1e-8], [1e-12, 1e-8, 1e-7], [1e-8, 1e-8, 1e-8], [1e-9, 1e-12, 1e-8],
+                                   [0.5, 0.5, 0.5], [0.4, 0.3, 0.5]])])
+    scl[:4, 0] = 1e-9                                 # a few fan Gaussians with one scale under the clamp
+    tilt = torch.cat([torch.ones(n_fan, 1), 0.2 * torch.randn(n_fan, 3, generator=g)], -1)
+    q = tilt / tilt.norm(dim=-1, keepdim=True) * torch.exp(0.7 * torch.randn(n_fan, 1, generator=g))
+    q = torch.cat([q, torch.tensor([[1.0, 0, 0, 0], [0.5, 0.5, 0.5, 0.5], [2.0, 0, 0, 0], [0, 0.3, 0, 0],
+                                    [1.5, 0.2, -0.4, 0.1], [0.7, 0, 0.7, 0]])])
+    strength = torch.cat([0.8 * torch.ones(n_fan), torch.tensor([LEVEL, 0.9, 0.9, 0.9, 0.8, 0.6])])[:, None]
+    gauss = (pts.float(), scl.float(), q.float(), strength.float())
+    assert gauss[3][n_fan, 0].item() == np.float32(LEVEL)
+    return dict(verts=verts.float(), faces=faces, gaussians=gauss, n_fan=n_fan)
+
+
+def _sphere_inputs():
+    sc = scenes.frosting_init_scene(600, 3000, 3000, 4)
+    g = torch.Generator().manual_seed(9)
+    q = sc["sugar"][2] * torch.exp(0.5 * torch.randn(len(sc["sugar"][2]), 1, generator=g))     # non-unit quaternions
+    return sc, (sc["sugar"][0], sc["sugar"][1], q, sc["sugar"][3])
+
+
+@pytest.mark.parametrize("mesh", ["sphere", "hand"])
+def test_normals_model_matches_the_float64_restatement(mesh):
+    m = hand_mesh() if mesh == "hand" else _sphere_inputs()[0]
+    n, raw = oracle.vertex_normals(m["verts"].numpy(), m["faces"].numpy())
+    want = scenes.p3d_verts_normals(m["verts"].double(), m["faces"]).numpy()
+    np.testing.assert_allclose(n.v, want, rtol=0, atol=1e-12)
+    assert np.isfinite(n.m).all() and (n.m > 0).any()
+    if mesh == "hand":
+        for v in (ISOLATED,) + ZERO_AREA:
+            assert (raw[v] == 0).all() and (n.v[v] == 0).all(), v
+        assert (n.v[0] == want[0]).all() and n.v[0, 2] > 0.99
+    # the magnitude covers the float32 restatement's rounding
+    n32 = scenes.p3d_verts_normals(m["verts"], m["faces"]).numpy()
+    assert (np.abs(n32 - n.v) <= 4 * oracle.ULP * n.m + 1e-30).all()
+
+
+@pytest.mark.parametrize("std_K", [1, 4, 32])
+def test_proposal_model_matches_the_float64_restatement(std_K):
+    """|s * (q^-1 (0, n) q)| averaged over the std_K nearest SuGaR Gaussians, q raw and not unit, as torch_initial_shell
+    restates pytorch3d's quaternion_apply and quaternion_invert."""
+    sc, sugar = _sphere_inputs()
+    n32 = scenes.p3d_verts_normals(sc["verts"], sc["faces"])
+    std_idx = oracle_knn(sc["verts"].numpy(), sugar[0].numpy(), std_K)
+    inner, outer, _ = oracle.proposal(n32.numpy(), sugar[1].numpy(), sugar[2].numpy(), std_idx, 3.0)
+    stds = lambda dt: (sugar[1].to(dt)[std_idx] * scenes.quaternion_apply(
+        scenes.quaternion_invert(sugar[2].to(dt)[std_idx]), n32.to(dt)[:, None])).norm(dim=-1).mean(dim=-1)
+    want = (3.0 * stds(torch.float64)).numpy()
+    np.testing.assert_allclose(inner.v, want, rtol=1e-12, atol=0)
+    np.testing.assert_allclose(outer.v, -want, rtol=1e-12, atol=0)
+    got32 = (3.0 * stds(torch.float32)).numpy()
+    assert (np.abs(got32 - inner.v) <= 4 * oracle.ULP * inner.m).all()
+
+
+def _staged(g, verts, normals, inner, outer, knn, n_samples, **kw):
+    fr = torch.linspace(0, 1, n_samples, dtype=torch.float64).numpy()
+    return oracle.level_stage(tuple(t.numpy() for t in g), verts.numpy(), normals.numpy(), inner.numpy(),
+                              outer.numpy(), knn, fr, **kw)
+
+
+def test_staged_level_model_matches_the_float64_restatement_on_the_edge_scene():
+    sc = edge_scene()
+    ref = edge_oracle(sc)
+    st = _staged(sc["gaussians"], sc["verts"], sc["normals"], sc["inner"], sc["outer"], sc["knn_idx"], N_SAMPLES,
+                 level=LEVEL, min_layer=MIN_LAYER, half_layer=MIN_LAYER / 2, min_clamp_inner=sc["clamp_inner"].numpy(),
+                 max_clamp_outer=sc["clamp_outer"].numpy())
+    np.testing.assert_allclose(st["d"].v, ref["d"], rtol=1e-12, atol=1e-15)
+    np.testing.assert_allclose(st["outer"].v, ref["outer_raw"], rtol=0, atol=1e-12)
+    np.testing.assert_allclose(st["inner"].v, ref["inner_raw"], rtol=0, atol=1e-12)
+    at = {n: i for i, n in enumerate(sc["names"])}
+    assert st["clamped_inner"][at["clamp_inner"]] and st["clamped_outer"][at["clamp_outer"]]
+    assert st["clamped_inner"].sum() == st["clamped_outer"].sum() == 1
+    assert (st["empty"] == ref["empty"]).all() and (st["flat"] == ref["flat"]).all() and st["saturated"].any()
+
+
+def test_staged_model_matches_the_float64_restatement_on_a_sphere():
+    """Normals, proposal and the first pass composed in float64 against torch_reference in float64, and the float32
+    restatement inside the magnitudes."""
+    sc, sugar = _sphere_inputs()
+    v = sc["verts"]
+    n, _ = oracle.vertex_normals(v.numpy(), sc["faces"].numpy())
+    std_idx, knn = oracle_knn(v.numpy(), sugar[0].numpy(), 4), oracle_knn(v.numpy(), sugar[0].numpy(), 16)
+    inner, outer, _ = oracle.proposal(n.v, sugar[1].numpy(), sugar[2].numpy(), std_idx, 3.0)
+    d64 = lambda x: torch.from_numpy(np.asarray(x, np.float64))
+    args = dict(n_samples=N_SAMPLES, K=16, level=LEVEL, min_layer_size=0.001, spatial_extent=4.0, knn_idx=d64(knn).long())
+    ref, dens = torch_reference(tuple(t.double() for t in sugar), v.double(), d64(n.v), d64(inner.v), d64(outer.v),
+                                return_densities=True, **args)
+    st = _staged(sugar, v.double(), d64(n.v), d64(inner.v), d64(outer.v), knn, N_SAMPLES, level=LEVEL,
+                 min_layer=0.004, half_layer=0.002)
+    np.testing.assert_allclose(st["d"].v, dens.numpy(), rtol=1e-10, atol=1e-14)
+    np.testing.assert_allclose(st["outer"].v, ref.outer_dist.numpy(), rtol=0, atol=1e-10)
+    np.testing.assert_allclose(st["inner"].v, ref.inner_dist.numpy(), rtol=0, atol=1e-10)
+    assert 0 < (st["first"] > 0).sum() < len(v)
+
+
+def test_hand_mesh_exact_level_in_the_model():
+    """At the isolated vertex every sample is the vertex and its density is exactly the level: not above, not under."""
+    m = hand_mesh()
+    g = m["gaussians"]
+    n, _ = oracle.vertex_normals(m["verts"].numpy(), m["faces"].numpy())
+    knn = oracle_knn(m["verts"].numpy(), g[0].numpy(), 4)
+    inner, outer, _ = oracle.proposal(n.v, g[1].numpy(), g[2].numpy(), knn, 3.0)
+    assert knn[ISOLATED, 0] == m["n_fan"] and inner.v[ISOLATED] == 0
+    st = oracle.level_stage(tuple(t.numpy() for t in g), m["verts"].numpy(), n.v, inner.v, outer.v, knn,
+                            torch.linspace(0, 1, N_SAMPLES).numpy(), level=oracle.f32(LEVEL),
+                            min_layer=oracle.f32(0.004), half_layer=oracle.f32(0.002))
+    assert (st["d"].v[ISOLATED] == oracle.f32(LEVEL)).all() and st["undecided"][ISOLATED].all()
+    assert not st["empty"][ISOLATED] and st["flat"][ISOLATED]
