@@ -15,6 +15,7 @@ from .sugar import SugarNeighbours, sample_in_gaussians, sdf_regularization
 from .sugar_dn import depth_normal_consistency, depth_normal_features
 from .knn import KNN, knn_points
 from .frosting_init import LevelPoints, initial_shell, level_points_along_normals
+from .frosting_create import GS_KEYS, Trimmed, create_frosting, trim_shell
 from .optim import FrostingAdam, OptimizationParams
 from .mesh import (MeshRasterizer, RasterizationSettings, Fragments, nvdiff_rasterization,
                    nvdiff_rasterization_with_pix_to_face, rasterize_mesh, gaussian_render_mask)
@@ -23,7 +24,7 @@ __all__ = [
     "GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "forward_with_state",
     "MeshRasterizer", "RasterizationSettings", "Fragments", "nvdiff_rasterization",
     "nvdiff_rasterization_with_pix_to_face", "rasterize_mesh", "gaussian_render_mask",
-    "install_as_diff_gaussian_rasterization", "frosting_attributes_fused", "frosting_render", "frosting_render_two_step", "FrostingEdit", "FrostingEditComplex", "frosting_render_edited", "FrostingSkin", "skin_tables", "TextureBaker", "compute_textured_mesh", "mesh_bary", "write_textured_obj", "l1_dssim_loss", "SugarNeighbours", "sample_in_gaussians", "sdf_regularization", "depth_normal_features", "depth_normal_consistency", "KNN", "knn_points", "LevelPoints", "initial_shell", "level_points_along_normals", "FrostingAdam", "OptimizationParams",
+    "install_as_diff_gaussian_rasterization", "frosting_attributes_fused", "frosting_render", "frosting_render_two_step", "FrostingEdit", "FrostingEditComplex", "frosting_render_edited", "FrostingSkin", "skin_tables", "TextureBaker", "compute_textured_mesh", "mesh_bary", "write_textured_obj", "l1_dssim_loss", "SugarNeighbours", "sample_in_gaussians", "sdf_regularization", "depth_normal_features", "depth_normal_consistency", "KNN", "knn_points", "LevelPoints", "initial_shell", "level_points_along_normals", "GS_KEYS", "Trimmed", "create_frosting", "trim_shell", "FrostingAdam", "OptimizationParams",
 ]
 
 

@@ -122,6 +122,23 @@ class FrostingInit(C.Structure):
                                           "d_densities")]
 
 
+TRIM_K = 8
+
+
+class FrostingCreate(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_verts", "n_faces", "n_iterations", "n_gaussians", "n_gs", "sh_rest",
+                                         "contract")] + \
+               [(n, C.c_float) for n in ("step", "inside_th", "extent", "min_height")] + \
+               [(n, C.c_void_p) for n in ("d_verts", "d_faces", "d_normals", "d_inner_init", "d_outer_init",
+                                          "d_inner_verts", "d_outer_verts", "d_inner_dist", "d_outer_dist",
+                                          "d_inner_stop", "d_outer_stop", "d_shell", "d_centres", "d_knn_workspace")] + \
+               [("knn_workspace_bytes", C.c_size_t)] + \
+               [(n, C.c_void_p) for n in ("d_knn_dists", "d_knn_idx", "d_camera_center", "d_volumes", "d_cells", "d_u",
+                                          "d_bary_logits", "d_points", "d_max_scales", "d_nn_idx", "d_sh_idx",
+                                          "d_gs_sh_dc", "d_gs_sh_rest", "d_dist2", "d_log_scales", "d_quats",
+                                          "d_opacity_logits", "d_sh_dc", "d_sh_rest")]
+
+
 ADAM_MAX_GROUPS = 16
 MAX_PEERS = 8
 PEER_HANDLE_BYTES = 64
@@ -183,7 +200,7 @@ ABI_STRUCTS = (
     ("fb200_extra", Extra), ("fb200_frosting_params", FrostingParams), ("fb200_frosting_grads", FrostingGrads),
     ("fb200_adam_args", AdamArgs), ("fb200_layout", Layout), ("fb200_frosting_edit", FrostingEdit),
     ("fb200_frosting_skin", FrostingSkin), ("fb200_texture", Texture), ("fb200_sugar_reg", SugarReg),
-    ("fb200_frosting_init", FrostingInit),
+    ("fb200_frosting_init", FrostingInit), ("fb200_frosting_create", FrostingCreate),
 )
 
 _i32, _i64, _f32, _vp, _int, _size = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_int, C.c_size_t
@@ -229,6 +246,10 @@ SIGNATURES = {
     "fb200_knn_workspace_bytes": (_size, [_i32, _i32, _i32]),
     "fb200_knn": (_int, [_vp, _i32, _vp, _i32, _i32, _vp, _size, _vp, _vp, _vp]),
     "fb200_level_points": (_int, [C.POINTER(FrostingInit), _vp]),
+    "fb200_frosting_trim": (_int, [C.POINTER(FrostingCreate), _vp]),
+    "fb200_frosting_volumes": (_int, [C.POINTER(FrostingCreate), _vp]),
+    "fb200_frosting_sample": (_int, [C.POINTER(FrostingCreate), _vp]),
+    "fb200_frosting_finish": (_int, [C.POINTER(FrostingCreate), _vp]),
     "fb200_adam_step": (_int, [C.POINTER(AdamArgs), _vp]),
     "fb200_peer_alloc": (_int, [_size, C.POINTER(_vp)]),
     "fb200_peer_free": (_int, [_vp]),

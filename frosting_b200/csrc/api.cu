@@ -298,7 +298,7 @@ int fb200_abi_struct_sizes(size_t* out) {
                                              sizeof(fb200_frosting_grads), sizeof(fb200_adam_args), sizeof(fb200_layout),
                                              sizeof(fb200_frosting_edit), sizeof(fb200_frosting_skin),
                                              sizeof(fb200_texture), sizeof(fb200_sugar_reg),
-                                             sizeof(fb200_frosting_init)};
+                                             sizeof(fb200_frosting_init), sizeof(fb200_frosting_create)};
     for (int i = 0; i < FB200_ABI_STRUCTS; ++i) out[i] = sizes[i];
     return FB200_OK;
 }
@@ -829,6 +829,84 @@ int fb200_level_points(const fb200_frosting_init* lp, void* stream) {
     int rc = check_level_points(lp);
     if (rc != FB200_OK) return rc;
     return check(launch_level_points(*lp, static_cast<cudaStream_t>(stream)), "level_points");
+}
+
+// fb200_frosting_*: extents, then the pointers each call reads or writes
+static int check_frosting_create(const fb200_frosting_create* c, const char* what) {
+    char msg[160];
+    if (!c) {
+        snprintf(msg, sizeof(msg), "%s: null struct", what);
+        return fail(FB200_EINVAL, msg);
+    }
+    if (c->n_verts < 0 || c->n_faces < 0 || c->n_iterations < 1 || c->n_gaussians < 0 || c->n_gs < 0 || c->sh_rest < 0) {
+        snprintf(msg, sizeof(msg), "%s: bad extents (V, F, N, n_gs, sh_rest >= 0, n_iterations >= 1)", what);
+        return fail(FB200_EINVAL, msg);
+    }
+    return FB200_OK;
+}
+
+static int missing(const char* what, const char* kind) {
+    char msg[160];
+    snprintf(msg, sizeof(msg), "%s: missing %s pointer", what, kind);
+    return fail(FB200_EINVAL, msg);
+}
+
+int fb200_frosting_trim(const fb200_frosting_create* c, void* stream) {
+    int rc = check_frosting_create(c, "frosting_trim");
+    if (rc != FB200_OK) return rc;
+    if (c->n_verts == 0) return FB200_OK;
+    if (c->n_faces < FB200_TRIM_K) return fail(FB200_EINVAL, "frosting_trim: the 8 nearest cells need F >= 8 faces");
+    if (!(c->inside_th >= 0.f) || !(c->step > 0.f)) return fail(FB200_EINVAL, "frosting_trim: inside_th >= 0 and step > 0");
+    if (!c->d_verts || !c->d_faces || !c->d_normals || !c->d_inner_init || !c->d_outer_init)
+        return missing("frosting_trim", "input");
+    if (!c->d_inner_dist || !c->d_outer_dist || !c->d_inner_stop || !c->d_outer_stop || !c->d_shell || !c->d_centres ||
+        !c->d_knn_workspace || !c->d_knn_dists || !c->d_knn_idx)
+        return missing("frosting_trim", "output");
+    if (misaligned(c->d_knn_workspace, 256)) return fail(FB200_EINVAL, "frosting_trim: the workspace must be 256-byte aligned");
+    if (c->knn_workspace_bytes < knn_workspace_bytes(c->n_faces, 2 * c->n_verts))
+        return fail(FB200_ENOSPC, "frosting_trim: workspace too small");
+    size_t need, reserved;
+    rc = check(knn_sort_scratch(c->n_faces, 2 * c->n_verts, &need, &reserved), "frosting_trim: radix-sort scratch query");
+    if (rc != FB200_OK) return rc;
+    if (need > reserved) return fail(FB200_ENOSPC, "frosting_trim: the workspace reserves too little radix-sort scratch");
+    return check(launch_frosting_trim(*c, static_cast<cudaStream_t>(stream)), "frosting_trim");
+}
+
+int fb200_frosting_volumes(const fb200_frosting_create* c, void* stream) {
+    int rc = check_frosting_create(c, "frosting_volumes");
+    if (rc != FB200_OK) return rc;
+    if (c->n_faces == 0) return FB200_OK;
+    if (!(c->min_height >= 0.f) || (c->contract && !(c->extent > 0.f)))
+        return fail(FB200_EINVAL, "frosting_volumes: min_height >= 0 and, contracting, extent > 0");
+    if (!c->d_verts || !c->d_faces || !c->d_inner_dist || !c->d_outer_dist || (c->contract && !c->d_camera_center))
+        return missing("frosting_volumes", "input");
+    if (!c->d_volumes) return missing("frosting_volumes", "output");
+    return check(launch_frosting_volumes(*c, static_cast<cudaStream_t>(stream)), "frosting_volumes");
+}
+
+int fb200_frosting_sample(const fb200_frosting_create* c, void* stream) {
+    int rc = check_frosting_create(c, "frosting_sample");
+    if (rc != FB200_OK) return rc;
+    if (c->n_gaussians == 0) return FB200_OK;
+    if (!c->d_faces || !c->d_inner_verts || !c->d_outer_verts || !c->d_cells || !c->d_u)
+        return missing("frosting_sample", "input");
+    if (!c->d_bary_logits || !c->d_points || !c->d_max_scales) return missing("frosting_sample", "output");
+    return check(launch_frosting_sample(*c, static_cast<cudaStream_t>(stream)), "frosting_sample");
+}
+
+int fb200_frosting_finish(const fb200_frosting_create* c, void* stream) {
+    int rc = check_frosting_create(c, "frosting_finish");
+    if (rc != FB200_OK) return rc;
+    if (c->n_gaussians == 0) return FB200_OK;
+    if (c->n_gaussians < 4 || c->n_gs < 1)
+        return fail(FB200_EINVAL, "frosting_finish: distCUDA2 needs N >= 4 Gaussians, the SH rows n_gs >= 1");
+    if (!c->d_points || !c->d_max_scales || !c->d_nn_idx || !c->d_sh_idx || !c->d_gs_sh_dc ||
+        (c->sh_rest > 0 && !c->d_gs_sh_rest))
+        return missing("frosting_finish", "input");
+    if (!c->d_dist2 || !c->d_log_scales || !c->d_quats || !c->d_opacity_logits || !c->d_sh_dc ||
+        (c->sh_rest > 0 && !c->d_sh_rest))
+        return missing("frosting_finish", "output");
+    return check(launch_frosting_finish(*c, static_cast<cudaStream_t>(stream)), "frosting_finish");
 }
 
 int fb200_adam_step(const fb200_adam_args* a, void* stream) {

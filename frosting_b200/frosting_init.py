@@ -150,16 +150,30 @@ def initial_shell(sugar, gs, verts, faces, spatial_extent, *, n_samples=21, K=16
     final_proposal_range and clamped to final_clamping_range of it.  `sugar` and `gs` are activated (points, scaling,
     quaternions, strengths); verts [V,3] float32 and faces [F,3] integer on one CUDA device.  Returns
     LevelPoints(outer_dist, inner_dist, outer_verts, inner_verts): Frosting's _outer_dist / _inner_dist and shell."""
+    return _initial_shell(sugar, gs, verts, faces, spatial_extent, n_samples=n_samples, K=K, level=level,
+                          smooth_K=smooth_K, min_frosting_size=min_frosting_size,
+                          initial_proposal_std_range=initial_proposal_std_range,
+                          final_proposal_range=final_proposal_range, final_clamping_range=final_clamping_range)[0]
+
+
+def _faces(faces, dev, V):
+    if not isinstance(faces, torch.Tensor) or faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point \
+            or faces.device != dev:
+        raise ValueError(f"faces must be an integer [F, 3] tensor on {dev}")
+    faces = faces.to(torch.int32).contiguous()
+    if faces.numel() and (int(faces.min()) < 0 or int(faces.max()) >= V):
+        raise ValueError(f"faces must index the {V} vertices")
+    return faces
+
+
+def _initial_shell(sugar, gs, verts, faces, spatial_extent, *, n_samples, K, level, smooth_K, min_frosting_size,
+                   initial_proposal_std_range, final_proposal_range, final_clamping_range):
+    """initial_shell's LevelPoints and the base mesh's vertex normals [V,3] it computed on the way."""
     dev = verts.device if isinstance(verts, torch.Tensor) else None
     with torch.no_grad():
         verts = _rows(verts, "verts", dev, 3)
         V = verts.shape[0]
-        if not isinstance(faces, torch.Tensor) or faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point \
-                or faces.device != dev:
-            raise ValueError(f"faces must be an integer [F, 3] tensor on {dev}")
-        faces = faces.to(torch.int32).contiguous()
-        if faces.numel() and (int(faces.min()) < 0 or int(faces.max()) >= V):
-            raise ValueError(f"faces must index the {V} vertices")
+        faces = _faces(faces, dev, V)
         gs_s, gs_v = _gaussians(sugar, dev), _gaussians(gs, dev)
         n_samples, K, smooth_K = int(n_samples), int(K), int(smooth_K)
         _extents(min(gs_s[0].shape[0], gs_v[0].shape[0]), K, n_samples, smooth_K, V)
@@ -180,7 +194,7 @@ def initial_shell(sugar, gs, verts, faces, spatial_extent, *, n_samples=21, K=16
         clamp_outer = centre + final_clamping_range * (surface.outer_dist - centre)
         clamp_inner = centre + final_clamping_range * (surface.inner_dist - centre)
         return _run(dev, verts, normals, gs_v, knn_points(verts, gs_v[0], K=K).idx, max_inner, min_outer, n_samples,
-                    level, smooth_idx, layer, clamp_inner, clamp_outer)
+                    level, smooth_idx, layer, clamp_inner, clamp_outer), normals
 
 
 def torch_reference(gaussians, verts, normals, inner_range, outer_range, *, n_samples=21, K=16, level, smooth_K=4,

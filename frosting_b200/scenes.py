@@ -877,3 +877,38 @@ def frosting_init_scene(n_verts, n_sugar, n_gs, seed, radius=2.0, centre=(0.0, 0
           torch.sigmoid(torch.randn(n_gs, 1, generator=g)))
     return dict(verts=verts, faces=faces, sugar=tuple(t.float().contiguous() for t in sugar),
                 gs=tuple(t.float().contiguous() for t in gs), spatial_extent=2.0 * radius)
+
+
+def frosting_create_scene(n_verts, n_sugar, n_gs, seed, radius=2.0, centre=(0.0, 0.0, 6.0), n_patch=32, bg_frac=0.05):
+    """frosting_init_scene plus what Frosting's constructor reads after the thickness: the 3DGS Gaussians as a
+    GaussianModel holds them raw (`gs_raw`: _xyz, _features_dc [P,1,3], _features_rest [P,15,3], _scaling (log),
+    _rotation, _opacity (logit) [P,1]), bg_frac of them moved outside the base mesh's bounding box (radius 3 to 5 times
+    `radius` around the centre), and a fold: a second sheet, an n_patch x n_patch grid on the sphere of radius 1.0005
+    `radius` over the cap within 0.25 rad of +x, normals outward, closer to the sphere than their shells are thick
+    (min_frosting_size alone makes them 0.001 * extent = 0.002 `radius`), so the two shells trim each other.
+    `camera_center` sits 1.5 `radius` from the centre along +z, so the faces beyond spatial_extent of it contract."""
+    sc = frosting_init_scene(n_verts, n_sugar, n_gs, seed, radius=radius, centre=centre)
+    g = torch.Generator().manual_seed(seed + 0x6372)
+    c = torch.tensor(centre)
+    s = torch.linspace(-0.25, 0.25, n_patch)
+    yy, zz = torch.meshgrid(s, s, indexing="ij")
+    d = torch.nn.functional.normalize(torch.stack([torch.ones_like(yy), torch.tan(yy), torch.tan(zz)], -1), dim=-1)
+    patch = c + 1.0005 * radius * d.reshape(-1, 3)
+    i = torch.arange(n_patch - 1)
+    a = (i[:, None] * n_patch + i[None, :]).reshape(-1)
+    V0 = len(sc["verts"])
+    # cross(v2 - v1, v0 - v1) along +x: (a, a + n, a + 1) and (a + 1, a + n, a + n + 1)
+    quads = torch.cat([torch.stack([a, a + n_patch, a + 1], 1), torch.stack([a + 1, a + n_patch, a + n_patch + 1], 1)])
+    verts = torch.cat([sc["verts"], patch.float()])
+    faces = torch.cat([sc["faces"], (quads + V0).int()])
+    pts, scaling, quats, strengths = sc["gs"]
+    P = len(pts)
+    n_bg = int(bg_frac * P)
+    pts = pts.clone()
+    u = torch.nn.functional.normalize(torch.randn(n_bg, 3, generator=g), dim=-1)
+    pts[:n_bg] = c + radius * (3.0 + 2.0 * torch.rand(n_bg, 1, generator=g)) * u
+    gs_raw = dict(_xyz=pts.contiguous(), _features_dc=torch.randn(P, 1, 3, generator=g),
+                  _features_rest=0.1 * torch.randn(P, 15, 3, generator=g), _scaling=scaling.log().contiguous(),
+                  _rotation=quats.contiguous(), _opacity=torch.logit(strengths).contiguous())
+    return dict(verts=verts.contiguous(), faces=faces.contiguous(), sugar=sc["sugar"], gs_raw=gs_raw,
+                spatial_extent=sc["spatial_extent"], camera_center=c + torch.tensor([0.0, 0.0, 1.5 * radius]))

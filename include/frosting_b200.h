@@ -572,6 +572,79 @@ typedef struct fb200_frosting_init {
 } fb200_frosting_init;
 int fb200_level_points(const fb200_frosting_init* lp, void* stream);
 
+/* Creating a Frosting layer from its thickness (frosting_model.py Frosting.__init__, :398-554, with
+ * avoid_self_intersections, contract_points and use_softmax_for_bary_coords).  Four calls over one struct, in order:
+ *   fb200_frosting_trim     the self-intersection trimming, n_iterations times: with d = 0 at first, every still active
+ *                           vertex side tries d + step * init (a float32 multiply, then an add); the trial shell vertex is
+ *                           vert + d n (multiply, then add) into d_shell [2V,3] (inner rows, then outer), each face's cell
+ *                           centre is the left-to-right sum of its 6 shell vertices (inner corners, then outer) over 6
+ *                           into d_centres; fb200_knn gives each of the 2V shell vertices its FB200_TRIM_K nearest
+ *                           centres (d_knn_*, workspace as fb200_knn_workspace_bytes(F, 2V, 8)); a vertex is inside a
+ *                           cell when all five projections (x - p_j) . n_j of is_inside_frosting (:1675-1737, n_j
+ *                           F.normalize(cross(...)) with eps 1e-12) exceed inside_th.  Inside any of its 8 cells: the side
+ *                           keeps its previous distance and stops (d_*_stop = the iteration); otherwise it takes the trial.
+ *                           Never stopped: d_*_stop = n_iterations.  Needs F >= 8;
+ *   fb200_frosting_volumes  d_volumes [F]: Heron's area of the face on contract(verts, camera centre, extent) times the
+ *                           mean over its vertices of max(|d_inner_dist - d_outer_dist|, min_height), times (extent / |vert
+ *                           - centre|)^2 beyond extent (contract = 0: plain vertices and heights);
+ *   fb200_frosting_sample   per Gaussian i in cell d_cells[i]: u = d_u[i] with u_5 = 1, sorted; b_0 = u_0, b_k = u_k -
+ *                           u_{k-1}; d_bary_logits = log(max(b, 1e-8)); d_points = sum_k b_k cell_k over the cell of
+ *                           d_inner_verts / d_outer_verts (inner corners, then outer); d_max_scales the longest of the
+ *                           cell's 3 sides and 6 base edges;
+ *   fb200_frosting_finish   d_dist2 = distCUDA2's ((b_0 + b_1) + b_2) / 3 over the neighbours d_nn_idx[i, 1..3] (a K = 4
+ *                           table over d_points, column 0 the point itself), each distance as simple-knn computes it for
+ *                           sm_90a, fmaf(dz, dz, fmaf(dx, dx, dy * dy)), ascending; d_log_scales [N,3] = log(sqrt(max(min(
+ *                           dist2, max_scale^2), 1e-7))); d_quats (1, 0, 0, 0); d_opacity_logits inverse_sigmoid(0.1);
+ *                           d_sh_dc / d_sh_rest the rows d_sh_idx[i] of d_gs_sh_dc [n_gs,3] / d_gs_sh_rest [n_gs,sh_rest,3].
+ * Tables are not checked and must lie in range.  Stream-ordered, no host synchronisation, no allocation, no atomics:
+ * the outputs depend on the input bits alone. */
+#define FB200_TRIM_K 8
+typedef struct fb200_frosting_create {
+    int32_t n_verts, n_faces, n_iterations, n_gaussians, n_gs, sh_rest, contract;
+    float step;                         /* 1 / n_iterations rounded to float32 */
+    float inside_th;                    /* spatial_extent * proj_th rounded to float32 */
+    float extent;                       /* spatial_extent rounded to float32 */
+    float min_height;                   /* min_frosting_size * spatial_extent rounded to float32 */
+    const float* d_verts;               /* [V,3] base mesh */
+    const int32_t* d_faces;             /* [F,3] */
+    const float* d_normals;             /* [V,3] */
+    const float* d_inner_init;          /* [V] the untrimmed distances */
+    const float* d_outer_init;          /* [V] */
+    const float* d_inner_verts;         /* [V,3] the untrimmed shell */
+    const float* d_outer_verts;         /* [V,3] */
+    float* d_inner_dist;                /* [V] trimmed (trim writes, volumes reads) */
+    float* d_outer_dist;                /* [V] */
+    int32_t* d_inner_stop;              /* [V] */
+    int32_t* d_outer_stop;              /* [V] */
+    float* d_shell;                     /* [2V,3] */
+    float* d_centres;                   /* [F,3] */
+    void* d_knn_workspace;
+    size_t knn_workspace_bytes;
+    float* d_knn_dists;                 /* [2V,8] */
+    int64_t* d_knn_idx;                 /* [2V,8] */
+    const float* d_camera_center;       /* [3] */
+    float* d_volumes;                   /* [F] */
+    const int64_t* d_cells;             /* [N] */
+    const float* d_u;                   /* [N,6] */
+    float* d_bary_logits;               /* [N,6] */
+    float* d_points;                    /* [N,3] */
+    float* d_max_scales;                /* [N] */
+    const int64_t* d_nn_idx;            /* [N,4] */
+    const int64_t* d_sh_idx;            /* [N] */
+    const float* d_gs_sh_dc;            /* [n_gs,3] */
+    const float* d_gs_sh_rest;          /* [n_gs,sh_rest,3] */
+    float* d_dist2;                     /* [N] */
+    float* d_log_scales;                /* [N,3] */
+    float* d_quats;                     /* [N,4] */
+    float* d_opacity_logits;            /* [N] */
+    float* d_sh_dc;                     /* [N,3] */
+    float* d_sh_rest;                   /* [N,sh_rest,3] */
+} fb200_frosting_create;
+int fb200_frosting_trim(const fb200_frosting_create* c, void* stream);
+int fb200_frosting_volumes(const fb200_frosting_create* c, void* stream);
+int fb200_frosting_sample(const fb200_frosting_create* c, void* stream);
+int fb200_frosting_finish(const fb200_frosting_create* c, void* stream);
+
 /* Data-parallel gradient reduction fused with the Adam update (SURVEY.md row f3).  Replaces "all-reduce every
  * .grad, then torch.optim.Adam(l, lr=0.0, eps=1e-15).step()" (frosting_scene/frosting_optimizer.py:101,116-118) for
  * camera-sharded training.  All learnable tensors of a rank live in ONE flat fp32 parameter slab and their gradients
@@ -676,10 +749,11 @@ int64_t fb200_kernel_launches(void);
 const char* fb200_last_error(void);
 int fb200_abi_version(void);
 /* sizeof() of the ABI structs, in this order: {params, inputs, workspace, grads, extra, frosting_params,
- * frosting_grads, adam_args, layout, frosting_edit, frosting_skin, texture, sugar_reg, frosting_init}: lets a
+ * frosting_grads, adam_args, layout, frosting_edit, frosting_skin, texture, sugar_reg, frosting_init,
+ * frosting_create}: lets a
  * foreign-language binding verify its struct mirrors at load time.  `out` holds FB200_ABI_STRUCTS entries of this
  * header; structs are only ever appended to the list. */
-#define FB200_ABI_STRUCTS 14
+#define FB200_ABI_STRUCTS 15
 int fb200_abi_struct_sizes(size_t* out /* [FB200_ABI_STRUCTS] */);
 
 #ifdef __cplusplus
